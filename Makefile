@@ -1,6 +1,6 @@
-# vartrix_b200 -- build the sm_100a engine library (and the oracle used by the tests).
+# vartrix_b200 -- build the sm_90a (H100) engine library (and the oracle used by the tests).
 NVCC      ?= /usr/local/cuda/bin/nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 EXTRA     ?=
 NVCCFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wextra -Xptxas -v $(EXTRA)
 CSRC      := vartrix_b200/csrc

@@ -62,6 +62,7 @@ def parse_args(argv=None):
     ap.add_argument("--growth", type=float, default=2.0, help="e2e shards grow geometrically from --first-chunk by this factor (0: equal shards after the first)")
     ap.add_argument("--first-chunk", type=float, default=0.01, help="fraction of the candidates in the first (priming) shard")
     ap.add_argument("--min-shard", type=int, default=100_000, help="e2e shards are not made smaller than this many candidates (per-submit fixed costs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the triplets of the last timed `value` step as DIR/<name>.npy (float64, at most 64 MB)")
     return ap.parse_args(argv)
 
 
@@ -93,7 +94,7 @@ def describe(args, cfg, world, info, extra=None):
         "parallelism": (f"loci sharded over {world} GPU(s), {args.scaling} scaling; triplets gathered over NCCL "
                         f"({'to rank 0 with ncclSend/Recv' if args.gather == 'root' else 'allgatherv on every rank'}), overlapped with the next step; "
                         f"on the e2e path every rank copies its own row range to its host (h2d/d2h bytes are job totals)") if world > 1 else "1 GPU",
-        "l2_policy": "inputs larger than L2 (staged shard >> 126 MB), no explicit flush",
+        "l2_policy": "inputs larger than L2 (staged shard >> 50 MB), no explicit flush",
         "staging_layout": "vtx_batch2 (slim)" if args.layout == "slim" else "vtx_batch",
         "e2e_chunks": args.chunks, "e2e_first_chunk_frac": args.first_chunk, "e2e_chunk_growth_cap": args.growth, "host_cores_bound_to_gpu": len(os.sched_getaffinity(0)),
     }
@@ -239,7 +240,7 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md recipe)
+# clocks sampler
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -278,6 +279,28 @@ class ClockSampler:
                 pass
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "power_w_max": max(pw) if pw else None, "samples": len(sm), "reasons": sorted(reasons)}
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, trip):
+    """Write the triplet arrays a caller of the timed path receives (the count arrays only when the engine returns them)
+    and its three metrics as DIR/<name>.npy in float64.  Above DUMP_BYTES in all, every array keeps the same fixed, seeded
+    sample of entries (in order), so that two builds given the same arguments can be compared entry for entry."""
+    arrays = {n: getattr(trip, n) for n in ("row", "col", "ref_cnt", "alt_cnt", "unk_cnt", "val", "val2")}
+    arrays = {n: a for n, a in arrays.items() if a.size}
+    n = len(trip.row)
+    keep = slice(None)
+    cap = (DUMP_BYTES - 4096) // (8 * max(len(arrays), 1))          # 4 KB for the .npy headers and the metrics
+    if n > cap:
+        keep = np.sort(np.random.default_rng(0).choice(n, cap, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a[keep], np.float64))
+    np.save(os.path.join(out_dir, "metrics.npy"),
+            np.array([trip.metrics[k] for k in ("num_not_cell_bc", "num_non_umi", "num_scored")], np.float64))
+    return {"dir": out_dir, "n_triplets": n, "n_dumped": min(n, cap), "arrays": sorted(arrays) + ["metrics"]}
 
 
 def triplet_checksum(row, col, val):
@@ -454,6 +477,7 @@ def run_gpu(args):
     gather_flush()
     sampler = ClockSampler(local) if rank == 0 else None
     ms, sw_ms, launches, last, clocks = timed(step_device, args.steps, sampler)
+    dumped = dump_outputs(args.dump_outputs, eng.fetch(last)) if args.dump_outputs and rank == 0 else None
     total_pairs = n_pairs * world
     if world > 1:
         tp = torch.tensor([n_pairs], device="cuda", dtype=torch.int64); dist.all_reduce(tp); total_pairs = int(tp.item())
@@ -517,21 +541,15 @@ def run_gpu(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6.65 TB/s"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "H100 SXM data sheet, 3.35 TB/s (not a measured peak)"
         b_alg = vb.synth.algorithmic_bytes_per_pair(info)
-        traffic, traffic_src, alu_pct, tj_kernel = None, None, None, "vtx_k_sw_fold"
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "sw_kernel_traffic.json")))
-            traffic = tj["dram_bytes_per_pair"] * n_pairs; traffic_src = tj["source"]; alu_pct = tj.get("alu_pipe_active_pct")
-            tj_kernel = tj.get("kernel", tj_kernel)
-        except Exception:
-            pass
         sw_avg_ms = float(np.mean(sw_ms))
         achieved = n_pairs * b_alg / (sw_avg_ms / 1e3) / 1e9
         cells = info["read_len"] * 2 * (2 * 100 + 1)
         # the bound that actually binds: the ALU pipe.  DPX s16x2 instructions (and PRMT) occupy it for 2 cycles per warp
-        # and SMSP, 32-bit VIADD / IADD3 / LOP3 / SEL / ISETP for 1 (profiles/r01_dpx_microbench.txt).  Counted from the SASS
-        # of the kernel that took the work (DESIGN.md section 4):
+        # and SMSP, 32-bit VIADD / IADD3 / LOP3 / SEL / ISETP for 1 (tools/dpx_microbench.cu, profiles/h100_dpx_microbench.txt).
+        # Per step of the kernel that took the work (DESIGN.md section 4):
         #   folded kernel, tile = 4 pairs: main-pass warp-step (12 columns, forward | reverse halves) = 54 DPX + 19 -> 127
         #     cycles, (m + 7) steps; allele-column warp-step (19 rows) = 86 DPX + 28 -> 200 cycles, (L + 7) steps for L allele
         #     columns; boundary unpack 135; junction 199 (8 more, divergent, when the alleles differ in length)
@@ -546,7 +564,7 @@ def run_gpu(args):
         else:
             alu_cycles_per_pair = ((m + 7) * 128.0 + (m + 3) * 280.0) / 8.0
             model_kernel = "two-phase SW kernel vtx_k_sw_split<0>"
-        sm_mhz = (clocks or {}).get("sm_mhz") or float(peaks.get("sm_max_mhz", 1965.0))
+        sm_mhz = (clocks or {}).get("sm_mhz") or float(peaks.get("sm_max_mhz", (clocks or {}).get("sm_max_mhz") or 1980.0))
         dpx_peak = torch.cuda.get_device_properties(local).multi_processor_count * 4.0 * sm_mhz * 1e6
         dpx_ach = n_pairs * alu_cycles_per_pair / (sw_avg_ms / 1e3)
         extra = {"device_submits_per_step": len(dparts)}
@@ -561,18 +579,19 @@ def run_gpu(args):
                     "last_step_device_ms": {k: round(t_e[k], 3) for k in ("h2d_ms", "prep_ms", "sw_ms", "post_ms")}},
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "ncu_alu_pipe_active_pct": alu_pct,
-                         "peak_source": peak_src, "kernel": tj_kernel,
+                         "peak_source": peak_src, "kernel": "vtx_k_sw_fold",
                          "kernel_ms": sw_avg_ms, "algorithmic_bytes_per_pair": b_alg, "pairs_per_launch": n_pairs / max(len(dparts), 1),
                          "gcups": n_pairs * cells / (sw_avg_ms / 1e3) / 1e9,
                          "issue_bound": {"what": "ALU-pipe busy cycles/s of the %s (SASS model: %.0f SMSP-cycles per pair)" % (model_kernel, alu_cycles_per_pair),
                                          "tiles_per_kernel_class": tiles,
                                          "achieved": dpx_ach, "peak": dpx_peak, "frac": dpx_ach / dpx_peak,
-                                         "peak_source": "n_SM x 4 SMSPs x sampled SM clock; DPX = 2 cycles, VIADD = 1 (measured, profiles/r01_dpx_microbench.txt)"},
+                                         "peak_source": "n_SM x 4 SMSPs x sampled SM clock; DPX = 2 cycles, VIADD = 1 (tools/dpx_microbench.cu, profiles/h100_dpx_microbench.txt)"},
                          "note": "integer DP: ~540 cell updates per algorithmic byte, so the kernel is DPX-issue bound, not HBM "
                                  "bound (DESIGN.md); gcups = DP cell updates/s of the SW kernel alone"},
             "clocks": clocks,
         }
+        if dumped:
+            line["dump_outputs"] = dumped
         if gather_check is not None:
             line["gather_check"] = gather_check
         if not args.no_cpu_baseline:        # rank 0, also at N > 1 (the other ranks wait at the barrier below)

@@ -1,8 +1,8 @@
 /*
- * vartrix_b200.h -- C ABI of the B200-native per-locus read-scoring engine.
+ * vartrix_b200.h -- C ABI of the H100-native per-locus read-scoring engine.
  *
  * Drop-in boundary for the hot path of 10XGenomics/vartrix v1.1.22 (all file:line citations are into
- * /root/reference/src/main.rs).  The reference has no FFI seam of its own; the seam this ABI sits
+ * vartrix src/main.rs).  The reference has no FFI seam of its own; the seam this ABI sits
  * behind is the rayon block main.rs:279-291 (evaluate_chunk -> evaluate_rec -> evaluate_alns) plus the
  * serial merge main.rs:320-348.  A host (Rust via `extern "C"`, C++, Python ctypes) keeps doing what
  * main.rs does up to and including the record filters (VCF/FASTA/BAM decode, construct_haplotypes

@@ -1,13 +1,14 @@
 """CPU ORACLE (test infrastructure): pin the oracle against the reference's own golden matrices.
 
-Runs the seven regression cases of /root/reference/src/main.rs:1207-1466 through
+Runs the seven regression cases of vartrix src/main.rs:1207-1466 through
 oracle.pipeline (Python decode + C oracle) and compares every output with the committed
 golden `.mtx` as a (row, col) -> value set, exactly like the reference's
 `assert_eq!(seen.to_csr(), expected.to_csr())` (main.rs:1230-1232).
 
-Usage:  python -m oracle.check_goldens [reference_test_dir]      (default /root/reference/test)
+Usage:  python -m oracle.check_goldens [reference_test_dir]      (default tests/golden/ref_inputs)
 """
 import math
+import os
 import sys
 
 from . import pipeline as P
@@ -36,7 +37,10 @@ def same(a, b):
     return all((math.isnan(a[k]) and math.isnan(b[k])) or a[k] == b[k] for k in a)
 
 
-def main(test_dir="/root/reference/test"):
+REF_INPUTS = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "ref_inputs")
+
+
+def main(test_dir=REF_INPUTS):
     ok = True
     for name, lines, pre, bcs, mode, umi, g_out, g_ref in CASES:
         nr, nc, res, batch, _ = P.run_files(f"{test_dir}/{pre}.vcf", f"{test_dir}/{pre}.bam", f"{test_dir}/{pre}.fa",

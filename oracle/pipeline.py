@@ -1,6 +1,6 @@
 """CPU ORACLE (test infrastructure, NOT product code) -- file decode + orchestration.
 
-Pure-Python restatement of the host side of /root/reference/src/main.rs (`_main`, 163-418):
+Pure-Python restatement of the host side of vartrix src/main.rs (`_main`, 163-418):
 barcode loading, VCF slurp, haplotype construction, BAM region fetch + the four record filters,
 staging into the batch layout of ``vtx_oracle.h`` and hand-off to the C oracle
 (``libvtx_oracle.so``) for CB lookup, Smith-Waterman and aggregation.  Only tests/,

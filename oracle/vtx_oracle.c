@@ -1,7 +1,7 @@
 /*
  * vtx_oracle.c -- CPU ORACLE (test infrastructure, NOT product code).  See vtx_oracle.h.
  *
- * Every function cites the reference lines it restates (/root/reference/src/main.rs unless
+ * Every function cites the reference lines it restates (vartrix src/main.rs unless
  * another file is named).  Third-party arithmetic that is absent from the reference tree:
  *   - bio 0.30.0 (Cargo.lock:175-177) bio::alignment::pairwise::banded::Aligner::local,
  *     called at main.rs:898-901: restated here from the published algorithm (Gotoh affine

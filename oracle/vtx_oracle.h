@@ -2,7 +2,7 @@
  * vtx_oracle.h -- CPU ORACLE (test infrastructure, NOT product code).
  *
  * A plain-C restatement of the per-locus read-scoring path of 10XGenomics/vartrix
- * (reference: /root/reference/src/main.rs, v1.1.22).  Only tests/, __graft_entry__.smoke()
+ * (reference: vartrix src/main.rs, v1.1.22).  Only tests/, __graft_entry__.smoke()
  * and bench.py's cpu_baseline / --impl reference leg may load this library.  The product
  * (vartrix_b200/) never links, imports or executes anything in oracle/.
  *

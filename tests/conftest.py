@@ -9,12 +9,12 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-# the reference's own regression inputs and golden matrices (/root/reference/test, committed verbatim as test data)
+# the reference's own regression inputs and golden matrices (vartrix's test/ directory, committed verbatim as test data)
 REF_TEST_DIR = os.path.join(GOLDEN, "ref_inputs")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     # the engine library, the CLI and the oracle are built in-tree; build them if a fresh checkout has none
     import subprocess
     need = [os.path.join(ROOT, "vartrix_b200", "lib", "libvartrix_b200.so"), os.path.join(ROOT, "vartrix_b200", "bin", "vartrix_b200"),

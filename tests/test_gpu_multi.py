@@ -1,5 +1,5 @@
 """2-GPU test of the engine's own NCCL allgatherv (vtx_comm_init / vtx_gather / vtx_fetch).  Needs >= 2 CUDA
-devices (run under `gpurun --gpus 2`); skipped elsewhere.  The host-side protocol is covered on CPU by
+devices (run on a machine with two GPUs); skipped elsewhere.  The host-side protocol is covered on CPU by
 tests/test_dist_gloo.py."""
 import os
 import socket

@@ -1,5 +1,5 @@
-"""The reference's own regression suite (/root/reference/src/main.rs:1207-1466) through the product CLI on the GPU:
-the seven argv of `mod tests`, the reference's input files (tests/golden/ref_inputs = /root/reference/test verbatim)
+"""The reference's own regression suite (vartrix src/main.rs:1207-1466) through the product CLI on the GPU:
+the seven argv of `mod tests`, the reference's input files (tests/golden/ref_inputs = vartrix's test/ directory verbatim)
 and its twelve golden comparisons, compared the way the reference compares them -- as CSR matrices, i.e. as
 (row, col) -> value sets (main.rs:1230-1232).  BASELINE.json configs[0] is `test_coverage_matrices`."""
 import gzip

@@ -6,7 +6,7 @@ cd "$(dirname "$0")/.."
 mkdir -p build/variants
 for v in "$@"; do
   name=${v%%:*}; flags=${v#*:}
-  ( /usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC $flags -Xptxas -v \
+  ( /usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC $flags -Xptxas -v \
       -shared -o build/variants/lib_$name.so vartrix_b200/csrc/vtx_api.cu -ldl 2> build/variants/$name.log \
       || { echo "BUILD FAILED: $name"; tail -5 build/variants/$name.log; } ) &
   while [ "$(jobs -r | wc -l)" -ge 6 ]; do sleep 1; done

@@ -1,4 +1,4 @@
-// Pipe-throughput probe for the instructions of the SW inner loop (sm_100a).  Prints warp-instructions
+// Pipe-throughput probe for the instructions of the SW inner loop (sm_90a).  Prints warp-instructions
 // per cycle per SM for independent chains, 32 warps per SM.  Design aid, not part of the product.
 #include <cstdio>
 #include <cstdint>

@@ -3,7 +3,7 @@
 // This probe runs the same cell update (same device functions, same 20 warps/SM, 96-register budget) on registers only
 // and then adds the other ingredients of the step one at a time: the profile merge, the shared-memory profile loads,
 // the boundary shuffles, the boundary store.  Output: cycles per warp-step per SMSP.  Design aid, not product code.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o sw_loop_microbench tools/sw_loop_microbench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o sw_loop_microbench tools/sw_loop_microbench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""vartrix_b200 -- B200-native engine for the per-locus read-scoring path of 10XGenomics/vartrix.
+"""vartrix_b200 -- H100-native engine for the per-locus read-scoring path of 10XGenomics/vartrix.
 
 The product is the CUDA library behind include/vartrix_b200.h (csrc/); this package is its thin
 Python host mirror.  Importing it does not need a GPU; creating an Engine does."""

@@ -1,6 +1,6 @@
 // bam_reader.hpp -- BGZF + BAM + BAI region reader for the staging host (own DEFLATE decoder, zlib as the
 // fallback; htslib is not in this image).  Replaces what rust-htslib 0.36 / C htslib give the reference at
-// /root/reference/src/main.rs:262, 470 (IndexedReader::from_path), 822-829 (fetch + records),
+// vartrix src/main.rs:262, 470 (IndexedReader::from_path), 822-829 (fetch + records),
 // 742/753 (Record::aux), 793-796 (cigar), 896 (seq).  Region semantics = the htslib iterator: every
 // record of the contig with pos < end and bam_endpos > beg, in file order.
 #pragma once

@@ -1,5 +1,5 @@
 // inputs.hpp -- FASTA(.fai) windows, VCF records, barcode list, Matrix-Market / label writers for the
-// staging host.  Each piece cites the reference lines (/root/reference/src/main.rs) it stands in for.
+// staging host.  Each piece cites the reference lines (vartrix src/main.rs) it stands in for.
 #pragma once
 #include <zlib.h>
 
@@ -201,7 +201,7 @@ inline char* mtx_line(char* p, uint32_t row, uint32_t col, double v)
 }
 
 // The text of a large matrix is formatted by `threads` workers in blocks of 64 k triplets and written in order
-// (the serial formatter was 12x the GPU time of a 1 M-read job, profiles/r01_cli_e2e.json).
+// (a serial formatter takes many times the GPU time of the job).
 inline bool write_mtx(const std::string& path, uint64_t n_rows, uint64_t n_cols, uint64_t n, const uint32_t* row,
                       const uint32_t* col, const double* val, std::string* err, unsigned threads = 0)
 {

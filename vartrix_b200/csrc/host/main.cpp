@@ -1,4 +1,4 @@
-// vartrix_b200 CLI -- keeps the `vartrix` flag surface (/root/reference/src/main.rs:40-135) and the
+// vartrix_b200 CLI -- keeps the `vartrix` flag surface (vartrix src/main.rs:40-135) and the
 // `_main` flow (main.rs:163-418): inputs are decoded and filtered on host threads (stager.hpp), every shard
 // of loci is handed to the GPU engine through the C ABI (include/vartrix_b200.h), outputs are the same
 // Matrix-Market / label files.  `--dump-staged` stops after staging (no GPU needed; used by the tests).
@@ -54,7 +54,7 @@ struct Opts {
 
 void usage()
 {
-    puts("vartrix_b200 -- Variant assignment for single cell genomics (B200-native engine)\n"
+    puts("vartrix_b200 -- Variant assignment for single cell genomics (H100-native engine)\n"
          "USAGE: vartrix_b200 --vcf FILE --bam FILE --fasta FILE --cell-barcodes FILE [OPTIONS]\n"
          "  -v, --vcf FILE              Called variant file (VCF)\n"
          "  -b, --bam FILE              Cellranger BAM file\n"

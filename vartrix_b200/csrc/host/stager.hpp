@@ -1,4 +1,4 @@
-// stager.hpp -- the host half of evaluate_rec / evaluate_alns (/root/reference/src/main.rs:610-695,
+// stager.hpp -- the host half of evaluate_rec / evaluate_alns (vartrix src/main.rs:610-695,
 // 809-894): per VCF record build the haplotype windows, fetch the overlapping BAM records, apply the
 // four record filters and stage the survivors as one `vtx_batch` shard.  Alignment, barcode lookup, UMI
 // gate and aggregation happen on the GPU behind include/vartrix_b200.h.

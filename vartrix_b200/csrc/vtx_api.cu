@@ -798,7 +798,11 @@ int vtx_create(const vtx_config* cfg, vtx_ctx** out)
     cudaDeviceProp prop{};
     cudaError_t pe = cudaGetDeviceProperties(&prop, cfg->device);
     if (pe != cudaSuccess) { g_create_error = cudaGetErrorString(pe); delete ctx; return VTX_E_CUDA; }
-    if (prop.major < 9) { g_create_error = "vartrix_b200 needs DPX (sm_90+); built for sm_100a"; delete ctx; return VTX_E_UNSUPPORTED; }
+    if (prop.major != 9 || prop.minor != 0) {      // sm_90a code loads on compute capability 9.0 only
+        delete ctx;
+        return set_err(nullptr, VTX_E_UNSUPPORTED, "vartrix_b200 is built for sm_90a (H100, compute capability 9.0); device %d is %d.%d",
+                       cfg->device, prop.major, prop.minor);
+    }
     ctx->n_sm = prop.multiProcessorCount;
     if (cfg->stream) { ctx->stream = static_cast<cudaStream_t>(cfg->stream); ctx->own_stream = false; }
     else {

@@ -1,7 +1,7 @@
 // vtx_inflate.cuh -- raw DEFLATE (RFC 1951) decoder for BGZF members on the device: one warp per member.
 //
 // Replaces, for the staging path, what htslib's bgzf_read_block -> inflate does for the reference
-// (/root/reference/src/main.rs:822-829 through rust-htslib; SURVEY.md section 8(f)-1).  BGZF members are independent,
+// (vartrix src/main.rs:822-829 through rust-htslib; SURVEY.md section 8(f)-1).  BGZF members are independent,
 // <= 64 KiB of output each, with the uncompressed size in the gzip trailer -- thousands of them per shard of loci.
 //
 // A warp owns one member.  Lane 0 walks the bit stream (64-bit bit buffer refilled from 4-byte words, two-level lookup
@@ -325,10 +325,9 @@ __host__ __device__ inline int decode_batch(State& s, Tables& T, uint8_t* lens, 
 // the warp-level kernel
 // ---------------------------------------------------------------------------------------------------------------
 // Output goes straight to global memory: a match copy is a dependent L2 round trip and lane 0's symbol decode a chain of
-// dependent ALU and shared-memory operations (~1 k cycles per symbol either way), so a warp takes ~2.9 ms per 64 KB member --
-// and what buys throughput is the number of members in flight: 20 warps per SM hide each other's latencies (2 960 members per
-// wave, ~65 GB/s of inflated bytes when a call brings that many).  Tried and measured worse (round 2): the member's output
-// assembled in 64 KB of shared memory by a lone warp per CTA -- 1.7 ms per member, but only 2 CTAs fit an SM: 11 GB/s.
+// dependent ALU and shared-memory operations, so a warp takes milliseconds per 64 KB member -- and what buys throughput is
+// the number of members in flight: 20 warps per SM hide each other's latencies.  The alternative, the member's output
+// assembled in 64 KB of shared memory by a lone warp per CTA, is faster per member but fits only 2 CTAs on an SM.
 #ifndef VTX_INFLATE_PIPELINE
 #define VTX_INFLATE_PIPELINE 1
 #endif

@@ -1,4 +1,4 @@
-// vtx_pipeline.cuh -- the integer/byte kernels either side of Smith-Waterman (sm_100a).
+// vtx_pipeline.cuh -- the integer/byte kernels either side of Smith-Waterman (sm_90a).
 // HBM-bound scatter/gather work: one thread per element, coalesced 4/8-byte accesses, no host
 // synchronisation between stages (every size that depends on data stays on the device).
 //

@@ -2,7 +2,7 @@
 // BGZF stream (vtx_inflate.cuh), turned into the engine's candidate lists.
 //
 // Replaces, for a host that only reads the compressed file, what csrc/host/stager.hpp + bam_reader.hpp do on staging
-// threads and the reference does through rust-htslib (/root/reference/src/main.rs:822-865, 737-757, 790-806):
+// threads and the reference does through rust-htslib (vartrix src/main.rs:822-865, 737-757, 790-806):
 //   fetch          every record of the contig with pos < end and bam_endpos > start, in file order   (main.rs:822-829)
 //   record filters mapq, --primary-alignments, --no-duplicates, useful_alignment, in that order      (main.rs:833-865)
 //   tags           CB (or --bam-tag) and UB: first aux field of that name, type Z                      (main.rs:737-757)

@@ -1,7 +1,7 @@
-// vtx_sw.cuh -- Smith-Waterman kernels (sm_100a) of the vartrix read-scoring path.
+// vtx_sw.cuh -- Smith-Waterman kernels (sm_90a) of the vartrix read-scoring path.
 //
 // Replaces bio::alignment::pairwise::banded::Aligner::local x2 per (read, locus) pair
-// (/root/reference/src/main.rs:898-901) and fuses evaluate_scores (main.rs:1019-1030) plus the
+// (vartrix src/main.rs:898-901) and fuses evaluate_scores (main.rs:1019-1030) plus the
 // count-matrix increment as an epilogue.  Integer DP, no tensor cores:
 //
 //  * ref and alt haplotype scores travel in the two int16 lanes of one 32-bit word (biased by kBias, see
@@ -47,11 +47,9 @@ constexpr uint32_t kNEG2 = pack2(0, 0);                             // biased -1
 constexpr uint32_t kGoeAdd = (uint32_t(uint16_t(int16_t(kGoe - 1))) << 16) | uint32_t(uint16_t(int16_t(kGoe)));   // + (gap, gap) incl. the carry
 // Cell update.  1 (default): the diagonal add rides inside VIADDMNMX, x = max(diag + s, F), and the floor of local
 // alignment joins the H maximum, h = VIMNMX3(x, E, 0).  0: round-1 form, tf = VIMNMX3(diag + s, F, 0), h = VIMNMX(tf, E).
-// Measured on B200 (profiles/r02_dpx_microbench.txt): 3-input DPX instructions hold the ALU pipe for 2 cycles, the 2-input
-// VIMNMX for 1, and a plain add next to a DPX instruction is free -- so form 1 costs 12 more ALU cycles per main-pass step
-// of the folded kernel (126 instead of 114) but 5 fewer issue slots (117 instead of 122), and the kernel is bound by both
-// (ncu: issue slots 81 % busy, ALU pipe 76 %).  Form 1 measured +1.9 %, with the row loop unrolled twice +3.7 %
-// (profiles/r02_fold_variants.txt).
+// On H100 (profiles/h100_dpx_microbench.txt) 3-input DPX instructions hold the ALU pipe for 2 cycles, the 2-input VIMNMX
+// for 1, and a plain add next to a DPX instruction is free -- so form 1 costs 12 more ALU cycles per main-pass step of the
+// folded kernel (126 instead of 114) but 5 fewer issue slots (117 instead of 122); the kernel is bound by both.
 #ifndef VTX_SW_FUSE
 #define VTX_SW_FUSE 1
 #endif
@@ -104,8 +102,8 @@ constexpr int kTileChunk = 8;            // most tiles grabbed per atomic
 // fast tile classes: lanes per pair, columns per lane, storage stride (words; CS % 4 == 0, (CS/4) odd
 // so the 8 lanes of an LDS.128 wavefront hit 8 distinct 16-byte bank groups)
 template <int CLS> struct TileClass;
-// THREADS x MINB = CTA shape / CTAs per SM the register allocator must leave room for (measured on B200,
-// profiles/r01_sw_variants.txt: 20 warps/SM at <= 102 registers beats 16 warps at 108 by ~4 %)
+// THREADS x MINB = CTA shape / CTAs per SM the register allocator must leave room for (the common classes:
+// 20 warps/SM, which leaves each thread <= 102 of the SM's 64 K registers)
 template <> struct TileClass<0> { static constexpr int LPP = 8, C = 26, CS = 28, THREADS = 320, MINB = 2; };   // n <= 208 (SNV, pad 100)
 template <> struct TileClass<1> { static constexpr int LPP = 8, C = 29, CS = 36, THREADS = 320, MINB = 2; };   // n <= 232 (indels <= 30)
 template <> struct TileClass<2> { static constexpr int LPP = 8, C = 32, CS = 36, THREADS = 256, MINB = 2; };   // n <= 256

@@ -1,7 +1,7 @@
 // vtx_sw_band.cuh -- VTX_BAND_MODEL: Smith-Waterman restricted to a k-mer-chain band (optional, slow path).
 //
 // The reference aligns with bio 0.30.0's banded::Aligner::new(GAP_OPEN, GAP_EXTEND, score, K = 6, W = 20).local(read, hap)
-// (/root/reference/src/main.rs:27-38, 898-901).  The crate's source is not available to this project; SURVEY.md
+// (vartrix src/main.rs:27-38, 898-901).  The crate's source is not available to this project; SURVEY.md
 // Appendix B restates its band from documentation and memory ("model B", the variant consistent with every golden of the
 // reference), and this kernel computes exactly that model:
 //   1. every exact k-mer hit (i, j): read[i .. i+k) == hap[j .. j+k), in (i, j) order            (byte equality)

@@ -1,6 +1,6 @@
 // vtx_sw_fold.cuh -- "folded" Smith-Waterman: neither shared flank of a locus is computed per haplotype.
 //
-// construct_haplotypes (/root/reference/src/main.rs:958-994) gives the ref and the alt window the SAME left
+// construct_haplotypes (vartrix src/main.rs:958-994) gives the ref and the alt window the SAME left
 // flank and the SAME right flank; only the allele columns in between differ.  The local-alignment maximum
 // decomposes exactly (oracle/vtx_oracle.c::vtxo_sw_fold pins this on the CPU against the full matrix):
 //
@@ -43,9 +43,8 @@ constexpr int kFoldMaxMid = 40;        // allele columns: n <= 2 * 96 + 40 = 232
 // (152 rows x 8 bytes put reads 0/2 and 1/3 on the same banks: a 2-way conflict on every boundary store and load)
 constexpr int kFoldRows = kFoldMaxRead + 4;
 constexpr int kFoldCodeStride = kFoldMaxRead + 16;   // row codes per read and direction (8 sentinels either side)
-// 288 threads x 2 CTAs = 18 warps/SM at 96 registers (a few spills in the tile prologue only).  Round 1 (unfused cell, no
-// unrolling): 320 x 2 beat 256 x 2 by 5 %; with the fused cell and the row loop unrolled twice 288 x 2 is the best of
-// 256 / 288 / 320 by ~1 % (profiles/r02_fold_variants.txt): the kernel is bound by issue slots and the ALU pipe, not by latency.
+// 288 threads x 2 CTAs = 18 warps/SM at 96 registers (a few spills in the tile prologue only); the kernel is bound by issue
+// slots and the ALU pipe, not by latency, so more resident warps buy little and fewer registers would cost spills.
 #ifndef VTX_FOLD_UNROLL
 #define VTX_FOLD_UNROLL 2
 #endif

@@ -1,7 +1,7 @@
 // vtx_sw_split.cuh -- two-phase Smith-Waterman that does not compute the shared left flank twice.
 //
 // The ref and alt haplotypes of a locus are identical up to the variant (construct_haplotypes,
-// /root/reference/src/main.rs:958-994: same left flank), so in the first kSplitP columns the two int16
+// vartrix src/main.rs:958-994: same left flank), so in the first kSplitP columns the two int16
 // halves of vtx_k_sw_pairs carry the same numbers.  Here a warp tile is 8 pairs of one locus:
 //
 //   phase 1  columns [0, 96): the two halves hold two DIFFERENT READS (A, B) against the common prefix.
@@ -26,7 +26,7 @@ constexpr int kSplitMaxRead = 256;     // longer reads use the single-phase clas
 template <int SCLS> struct SplitClass;
 // COPIES: 2 = the phase-2 profile is stored twice, 16 banks apart, so the two reads of an LDS wavefront never
 // collide; 1 = single copy (2-way conflicts on those loads, 3 KB less shared memory per warp)
-// defaults = the best of profiles/r01_split_variants.txt (B200): one copy and 20 warps/SM for the SNV class
+// defaults: one copy and 20 warps/SM for the SNV class (the shared memory of a second copy costs resident warps)
 #ifndef VTX_SPLIT0_COPIES
 #define VTX_SPLIT0_COPIES 1
 #endif

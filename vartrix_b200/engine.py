@@ -1,7 +1,7 @@
 """Python host mirror of the engine's C ABI (used by the tests and bench.py; a production host is
 the C++ CLI in csrc/host or any FFI binding of include/vartrix_b200.h).
 
-Names follow the reference (``/root/reference/src/main.rs``): a *locus* is one VCF record, a
+Names follow the reference (``vartrix src/main.rs``): a *locus* is one VCF record, a
 *candidate* one BAM record fetched for a locus that passed the record filters (main.rs:833-865), a
 *pair* a candidate whose cell barcode is in the barcode list (main.rs:867-877) -- the unit that
 reaches the aligner (main.rs:896-930).

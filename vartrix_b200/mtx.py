@@ -1,5 +1,5 @@
 """Matrix Market text exactly as sprs 0.7.1 `write_matrix_market` emits it for the reference
-(/root/reference/src/main.rs:381-389; layout observed in every golden, SURVEY.md A.9):
+(vartrix src/main.rs:381-389; layout observed in every golden, SURVEY.md A.9):
 header, `% written by sprs`, `rows cols nnz`, then `row+1 col+1 value` in insertion order with the
 value printed like Rust's `{}` for f64 (shortest round-trip digits, never an exponent, `NaN`)."""
 from __future__ import annotations
