@@ -63,6 +63,33 @@ def test_slim_exotic_tags_missing_tags_shared_reads_ragged_lengths(oracle):
         sl, got = _both(oracle, sb2, bcs2, mode, use_umi, parts)
         assert sl.n_exotic > 100 and sl.cand_read is not None
         assert got.metrics["num_not_cell_bc"] > 60
+        # the same shards resident on the device (vtx_submit2_device): the host must not read their arrays
+        res = _resident(sl, sb2.cand_start, bcs2, mode, use_umi, parts)
+        assert_same_triplets(res, got)
+        assert res.metrics == got.metrics
+
+
+def _resident(sl, cand_start, bcs, mode, umi, n_parts):
+    """Every shard copied to the device with torch and submitted through vtx_submit2_device."""
+    import torch
+    import vartrix_b200 as vb
+    max_read = int(sl.read_len.max())
+    max_hap = int(max(sl.ref_len.max(), sl.alt_len.max()))
+    keep = []
+    with vb.Engine(mode, umi=umi) as eng:
+        eng.set_barcodes(bcs)
+        for lo, hi in vb.shard_bounds(cand_start, n_parts):
+            part = sl.shard(lo, hi) if n_parts > 1 else sl
+            ptr = {}
+            for f in vb.SlimBatch.ARRAYS:
+                a = getattr(part, f)
+                if a is None or a.size == 0:
+                    continue
+                t = torch.from_numpy(a.view(np.uint8).reshape(-1) if a.dtype.itemsize > 1 else a.reshape(-1)).cuda()
+                keep.append(t)
+                ptr[f] = t.data_ptr()
+            eng.submit2_device(part.to_c(ptr), max_read, max_hap)
+        return eng.finish()
 
 
 def test_slim_empty_shards(oracle):

@@ -116,6 +116,11 @@ def test_header_symbols_are_exported():
     for s in _capi.SYMBOLS:
         assert hasattr(lib, s), s
     assert lib.vtx_abi_version() == 2
+    # ... and nothing else: internal helpers must not leak into the library's C interface
+    import subprocess
+    nm = subprocess.run(["nm", "-D", "--defined-only", _capi.LIB_PATH], check=True, capture_output=True, text=True).stdout
+    exported = {ln.split()[-1] for ln in nm.splitlines() if ln.split() and ln.split()[-1].startswith("vtx_")}
+    assert exported == declared, exported ^ declared
 
 
 def test_header_is_plain_c(tmp_path):

@@ -10,6 +10,7 @@
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
 #include <algorithm>
+#include <array>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -30,8 +31,47 @@ struct Nvtx {
 };
 constexpr int kBandK = 6, kBandW = 20;       // K, W of banded::Aligner::new (main.rs:33-34, 899)
 
+// device memory owned by the context: freed with it, grown by ensure()
 struct DBuf {
     void* p = nullptr;
+    size_t cap = 0;
+    DBuf() = default;
+    DBuf(const DBuf&) = delete;
+    DBuf& operator=(const DBuf&) = delete;
+    ~DBuf() { release(); }
+    cudaError_t release()
+    {
+        const cudaError_t e = p ? cudaFree(p) : cudaSuccess;
+        p = nullptr; cap = 0;
+        return e;
+    }
+    void swap(DBuf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
+};
+
+// pinned host memory owned by the context
+struct HostBuf {
+    void* p = nullptr;
+    HostBuf() = default;
+    HostBuf(const HostBuf&) = delete;
+    HostBuf& operator=(const HostBuf&) = delete;
+    ~HostBuf() { release(); }
+    void release() { if (p) cudaFreeHost(p); p = nullptr; }
+    cudaError_t alloc(size_t bytes, unsigned flags = cudaHostAllocDefault)
+    {
+        release();
+        const cudaError_t e = cudaHostAlloc(&p, bytes, flags);
+        if (e != cudaSuccess) p = nullptr;
+        return e;
+    }
+    template <typename T> T* as() const { return static_cast<T*>(p); }
+};
+
+// The seven triplet arrays of a result, in vtx_result order: row, col, ref_cnt, alt_cnt, unk_cnt, val, val2.
+constexpr int kResArrays = 7;
+constexpr size_t kResEsz[kResArrays] = { 4, 4, 4, 4, 4, 8, 8 };
+
+struct HostResults {    // pinned host copies of the result arrays, room for `cap` triplets
+    HostBuf a[kResArrays];
     size_t cap = 0;
 };
 
@@ -87,7 +127,7 @@ struct vtx_ctx {
     cudaStream_t stage_stream = nullptr;
     DBuf bam_metrics;                                   // stage::LocusMetrics, cumulative
     DBuf stage_sums;                                    // block sums of the scans on the staging stream
-    uint64_t* h_stage = nullptr;                        // pinned scalars read back between the staging phases
+    HostBuf h_stage;                                    // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
 
@@ -100,18 +140,17 @@ struct vtx_ctx {
         pair_first, pair_cslot, pair_uslot, cslot_col, cslot_locus, uslot_cslot, ccnt, ucnt, keep2, oidx, tile_counters,
         scratch, pair_scores, d_metrics, d_res_n, big_list, slot_scratch;
     // results (device) + host mirrors
-    DBuf r_row, r_col, r_ref, r_alt, r_unk, r_val, r_val2;
+    DBuf res[kResArrays];
     size_t res_cap = 0;        // entries
     size_t res_ub = 0;         // upper bound of entries currently held
     bool finished = true;      // true: next submit starts a fresh result set
-    void* h_res[7] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
-    size_t h_res_cap = 0;
-    void* h_scalars = nullptr; // pinned: res_n (u64) + 3 metrics (u64)
+    HostResults h_res;
+    HostBuf h_scalars;         // res_n (u64) + 3 metrics (u64)
     uint64_t last_n = 0;
     vtx_metrics last_metrics{};
 
     cudaStream_t fetch_stream = nullptr;                 // device->host copies of finished triplets
-    unsigned long long* h_cum = nullptr;                 // host-mapped running triplet count after each submit
+    HostBuf h_cum;                                       // host-mapped running triplet count after each submit
     unsigned long long* d_cum = nullptr;                 // device alias of h_cum
     std::vector<TimeRec> trecs;     // one per submit since the last finish (events are reused)
     size_t trec_used = 0;
@@ -120,16 +159,15 @@ struct vtx_ctx {
     bool last_tiles_valid = false;
     uint64_t t_pairs = 0;
 
-    // multi-GPU (vtx_comm.cpp)
+    // multi-GPU (vtx_comm_init / vtx_gather_start)
     void* comm = nullptr;
     int rank = 0, n_ranks = 1;
-    void* g_host[7] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
-    size_t g_host_cap = 0;
-    DBuf g_dev[7];
+    HostResults g_host;
+    DBuf g_dev[kResArrays];
     DBuf g_counts;
     cudaStream_t comm_stream = nullptr;          // the gather runs here so that later submits overlap it
     cudaEvent_t ev_counts = nullptr, ev_gather = nullptr, ev_results = nullptr;
-    uint64_t* h_counts = nullptr;                // pinned: [n_ranks + 1][4]
+    HostBuf h_counts;                            // [n_ranks + 1][4]
     bool gather_pending = false;                 // started, not yet waited for
     bool gather_guard = false;                   // ev_gather must be awaited (on the device) before r_* are overwritten
     vtx_result g_out{};
@@ -158,7 +196,7 @@ int ensure(vtx_ctx* ctx, DBuf& b, size_t bytes)
     if (b.p) {
         CK(cudaStreamSynchronize(ctx->stream));
         if (ctx->copy_stream) CK(cudaStreamSynchronize(ctx->copy_stream));
-        CK(cudaFree(b.p)); b.p = nullptr; b.cap = 0;
+        CK(b.release());
     }
     size_t want = bytes + bytes / 8 + 256;
     cudaError_t e = cudaMalloc(&b.p, want);
@@ -186,16 +224,84 @@ TimeRec* new_trec(vtx_ctx* ctx)
 
 inline unsigned blocks_for(uint64_t n, unsigned threads) { return unsigned((n + threads - 1) / threads); }
 
-// exclusive scan wrapper: out has n + 1 entries
-int scan_u32(vtx_ctx* ctx, const uint32_t* in, uint64_t n, uint32_t* out, uint64_t* launches)
+// exclusive scan on stream `st` with block sums in `sums`: out has n + 1 entries
+int scan_u32(vtx_ctx* ctx, cudaStream_t st, DBuf& sums, const uint32_t* in, uint64_t n, uint32_t* out, uint64_t* launches)
 {
     const unsigned nb = std::max(1u, blocks_for(n, kScanTile));
-    ENS(ctx->scan_sums, size_t(nb) * 4);
-    vtx_k_scan_tiles<<<nb, kScanThreads, 0, ctx->stream>>>(in, n, out, P<uint32_t>(ctx->scan_sums));
-    vtx_k_scan_sums<<<1, kScanThreads, 0, ctx->stream>>>(P<uint32_t>(ctx->scan_sums), nb, out + n);
-    vtx_k_scan_add<<<nb, kScanThreads, 0, ctx->stream>>>(out, n, P<uint32_t>(ctx->scan_sums));
+    ENS(sums, size_t(nb) * 4);
+    vtx_k_scan_tiles<<<nb, kScanThreads, 0, st>>>(in, n, out, P<uint32_t>(sums));
+    vtx_k_scan_sums<<<1, kScanThreads, 0, st>>>(P<uint32_t>(sums), nb, out + n);
+    vtx_k_scan_add<<<nb, kScanThreads, 0, st>>>(out, n, P<uint32_t>(sums));
     if (launches) *launches += 3;
     CK(cudaGetLastError());
+    return VTX_OK;
+}
+
+// one warp per BGZF member; the decoder's tables and input windows need the opt-in shared-memory size
+int launch_inflate(vtx_ctx* ctx, cudaStream_t st, const void* desc, uint32_t n, const void* comp, void* out, void* status,
+                   uint32_t* cursor, int check_crc)
+{
+    using namespace inflate;
+    if (!ctx->inflate_attr_set) {
+        CK(cudaFuncSetAttribute(vtx_k_bgzf_inflate, cudaFuncAttributeMaxDynamicSharedMemorySize, int(inflate_smem_bytes())));
+        ctx->inflate_attr_set = true;
+    }
+    const unsigned ctas = unsigned(std::min<uint64_t>((n + kInflateWarps - 1) / kInflateWarps, uint64_t(ctx->n_sm) * 6));
+    vtx_k_bgzf_inflate<<<ctas, kInflateWarps * 32, inflate_smem_bytes(), st>>>(static_cast<const BlockDesc*>(desc), n,
+        static_cast<const uint8_t*>(comp), static_cast<uint8_t*>(out), static_cast<int32_t*>(status), cursor, check_crc);
+    CK(cudaGetLastError());
+    return VTX_OK;
+}
+
+// the result arrays that travel to the host: VTX_F_VALUES_ONLY keeps the three counts (and val2 outside coverage mode) on the device
+uint32_t want_mask(const vtx_ctx* ctx)
+{
+    const bool values_only = (ctx->cfg.flags & VTX_F_VALUES_ONLY) != 0;
+    return values_only ? (ctx->cfg.mode == VTX_MODE_COVERAGE ? 0x63u : 0x23u) : 0x7Fu;
+}
+
+template <typename Buf> std::array<const void*, kResArrays> ptrs(const Buf (&b)[kResArrays])
+{
+    std::array<const void*, kResArrays> a;
+    for (int i = 0; i < kResArrays; ++i) a[i] = b[i].p;
+    return a;
+}
+
+// points `out` at the arrays of `a` that `want` selects (NULL for the others)
+void point_result(vtx_result* out, const std::array<const void*, kResArrays>& a, uint32_t want, uint64_t n, const vtx_metrics& m)
+{
+    auto u32 = [&](int i) { return (want >> i & 1) ? static_cast<const uint32_t*>(a[i]) : nullptr; };
+    auto f64 = [&](int i) { return (want >> i & 1) ? static_cast<const double*>(a[i]) : nullptr; };
+    out->n = n;
+    out->row = u32(0); out->col = u32(1); out->ref_cnt = u32(2); out->alt_cnt = u32(3); out->unk_cnt = u32(4);
+    out->val = f64(5); out->val2 = f64(6);
+    out->metrics = m;
+}
+
+// pinned host result arrays with room for `n` triplets (only the wanted arrays are allocated)
+int ensure_host(vtx_ctx* ctx, HostResults& h, size_t n)
+{
+    if (n <= h.cap) return VTX_OK;
+    const size_t ncap = n + n / 4 + 1024;
+    const uint32_t want = want_mask(ctx);
+    for (int i = 0; i < kResArrays; ++i) {
+        h.a[i].release();
+        if (!(want >> i & 1)) continue;
+        const cudaError_t e = h.a[i].alloc(ncap * kResEsz[i]);
+        if (e != cudaSuccess) { h.cap = 0; return set_err(ctx, VTX_E_NOMEM, "pinned result alloc failed: %s", cudaGetErrorString(e)); }
+    }
+    h.cap = ncap;
+    return VTX_OK;
+}
+
+// device->host copy of entries [from, to) of the wanted result arrays
+int copy_results(vtx_ctx* ctx, HostResults& h, const std::array<const void*, kResArrays>& src, size_t from, size_t to, cudaStream_t st)
+{
+    const uint32_t want = want_mask(ctx);
+    for (int i = 0; i < kResArrays; ++i)
+        if ((want >> i & 1) && src[i])
+            CK(cudaMemcpyAsync(h.a[i].as<uint8_t>() + from * kResEsz[i], static_cast<const uint8_t*>(src[i]) + from * kResEsz[i],
+                               (to - from) * kResEsz[i], cudaMemcpyDeviceToHost, st));
     return VTX_OK;
 }
 
@@ -222,55 +328,34 @@ SwAllow sw_allow(const vtx_ctx* ctx, uint32_t max_read, uint32_t max_hap)
     a.fold = !(ctx->cfg.flags & (VTX_F_NO_SPLIT | VTX_F_NO_FOLD));
     return a;
 }
-template <int CLS>
-int launch_sw_class(vtx_ctx* ctx, SwArgs a, uint64_t* launches)
+// A persistent grid of a Smith-Waterman kernel: as many blocks as fit on every SM at once, each warp taking tiles from
+// a.tile_counter until none are left.  `name` / `cls` (-1: none) name the kernel in the error message.
+int launch_sw(vtx_ctx* ctx, void (*kern)(SwArgs), int threads, size_t warp_bytes, const SwArgs& a, uint64_t* launches,
+              const char* name, int cls)
 {
-    using TC = TileClass<CLS>;
-    constexpr int PPW = 32 / TC::LPP, RS = TC::LPP * TC::CS;
-    const size_t codes_bytes = (size_t(PPW) * (a.mcap + 2 * TC::LPP) * 2 + 7) & ~size_t(7);
-    const size_t bnd_bytes = (CLS == kMultiClass && a.multi) ? size_t(PPW) * (a.mcap + 8) * 8 : 0;
-    const size_t warp_bytes = (size_t(5 * RS) * 4 + codes_bytes + bnd_bytes + 15) & ~size_t(15);
-    constexpr int kSwThreads = TC::THREADS;
-    const size_t smem = warp_bytes * (kSwThreads / 32);
-    auto kern = vtx_k_sw_pairs<CLS>;
+    const size_t smem = warp_bytes * (threads / 32);
     CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
     int per_sm = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kSwThreads, smem));
-    if (per_sm < 1) return set_err(ctx, VTX_E_CUDA, "SW kernel class %d does not fit on an SM (smem %zu)", CLS, smem);
-    kern<<<ctx->n_sm * per_sm, kSwThreads, smem, ctx->stream>>>(a);
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    if (per_sm < 1) {
+        if (cls < 0) return set_err(ctx, VTX_E_CUDA, "%s does not fit on an SM (smem %zu)", name, smem);
+        return set_err(ctx, VTX_E_CUDA, "%s %d does not fit on an SM (smem %zu)", name, cls, smem);
+    }
+    kern<<<ctx->n_sm * per_sm, threads, smem, ctx->stream>>>(a);
     CK(cudaGetLastError());
     ++*launches;
     return VTX_OK;
 }
 
-template <int SCLS>
-int launch_sw_split(vtx_ctx* ctx, SwArgs a, uint64_t* launches)
+template <int CLS> int launch_sw_class(vtx_ctx* ctx, const SwArgs& a, uint64_t* launches)
 {
-    using SC = SplitClass<SCLS>;
-    const size_t smem = split_warp_bytes<SCLS>(a.mcap) * (SC::THREADS / 32);
-    auto kern = vtx_k_sw_split<SCLS>;
-    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    int per_sm = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SC::THREADS, smem));
-    if (per_sm < 1) return set_err(ctx, VTX_E_CUDA, "split SW kernel %d does not fit on an SM (smem %zu)", SCLS, smem);
-    kern<<<ctx->n_sm * per_sm, SC::THREADS, smem, ctx->stream>>>(a);
-    CK(cudaGetLastError());
-    ++*launches;
-    return VTX_OK;
+    return launch_sw(ctx, vtx_k_sw_pairs<CLS>, TileClass<CLS>::THREADS, sw_warp_bytes<CLS>(a.mcap, a.multi), a, launches,
+                     "SW kernel class", CLS);
 }
-
-int launch_sw_fold(vtx_ctx* ctx, SwArgs a, uint64_t* launches)
+template <int SCLS> int launch_sw_split(vtx_ctx* ctx, const SwArgs& a, uint64_t* launches)
 {
-    const size_t smem = fold_warp_bytes() * (kFoldThreads / 32);
-    auto kern = vtx_k_sw_fold;
-    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    int per_sm = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kFoldThreads, smem));
-    if (per_sm < 1) return set_err(ctx, VTX_E_CUDA, "folded SW kernel does not fit on an SM (smem %zu)", smem);
-    kern<<<ctx->n_sm * per_sm, kFoldThreads, smem, ctx->stream>>>(a);
-    CK(cudaGetLastError());
-    ++*launches;
-    return VTX_OK;
+    return launch_sw(ctx, vtx_k_sw_split<SCLS>, SplitClass<SCLS>::THREADS, split_warp_bytes<SCLS>(a.mcap), a, launches,
+                     "split SW kernel", SCLS);
 }
 
 // classes + tiles + SW kernels, shared by submit and score_pairs.  pair_start must be ready.
@@ -281,12 +366,10 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
     ENS(ctx->tcount, size_t(kNumClasses) * (nl + 1) * 4);
     ENS(ctx->tstart, size_t(kNumClasses) * (nl + 1) * 4);
     ENS(ctx->tile_counters, 64);
-    const int force_slow = 0;       // reads of any supported length run on the single-phase classes (row blocks)
-    const SwAllow allow = sw_allow(ctx, b.max_read_len, b.max_hap_len);
-    const int allow_split = allow.split, allow_multi = allow.multi, allow_fold = allow.fold;   // fold: per locus, windows and read lengths decide
+    const SwAllow allow = sw_allow(ctx, b.max_read_len, b.max_hap_len);     // fold: per locus, windows and read lengths decide
     vtx_k_locus_prep<<<blocks_for(uint64_t(nl) * 32, 256), 256, 0, ctx->stream>>>(
         nl, b.hap, b.ref_off, b.ref_len, b.alt_off, b.alt_len, P<uint32_t>(ctx->pair_start), P<uint32_t>(ctx->pair_read), b.read_len,
-        force_slow, allow_split, allow_multi, allow_fold, b.max_read_len, b.max_hap_len, P<unsigned long long>(ctx->d_metrics) + 4,
+        /*force_slow=*/0, allow.split, allow.multi, allow.fold, b.max_read_len, b.max_hap_len, P<unsigned long long>(ctx->d_metrics) + 4,
         P<uint32_t>(ctx->tcount));
     ++*launches;
     vtx_k_scan_rows<<<kNumClasses, kScanThreads, 0, ctx->stream>>>(P<uint32_t>(ctx->tcount), P<uint32_t>(ctx->tstart), nl, nl + 1);
@@ -308,7 +391,7 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
     a.mcap = mcap;
     a.k64k = 65536u;
     a.one = 1u;
-    a.multi = allow_multi;
+    a.multi = allow.multi;
     a.max_hap = b.max_hap_len;
 
     uint64_t before = *launches;
@@ -354,7 +437,7 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
         }
         if (rc) return rc;
     }
-    if (allow_split) {
+    if (allow.split) {
         for (int c = 0; c < kNumSplitClasses; ++c) {
             if (c > 0 && b.max_hap_len <= uint32_t(split_max_n(c - 1))) continue;
             if (!(b.class_mask >> (kSplitClass0 + c) & 1u)) continue;
@@ -364,10 +447,10 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
             if (rc) return rc;
         }
     }
-    if (allow_fold && (b.class_mask >> kFoldClass & 1u)) {
+    if (allow.fold && (b.class_mask >> kFoldClass & 1u)) {
         a.tile_start = P<uint32_t>(ctx->tstart) + size_t(kFoldClass) * (nl + 1);
         a.tile_counter = P<uint32_t>(ctx->tile_counters) + kFoldClass;
-        int rc = launch_sw_fold(ctx, a, launches);
+        int rc = launch_sw(ctx, vtx_k_sw_fold, kFoldThreads, fold_warp_bytes(), a, launches, "folded SW kernel", -1);
         if (rc) return rc;
     }
     if (b.class_mask >> kSlowClass & 1u) {   // generic class (rare)
@@ -382,7 +465,6 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
         ++*launches;
     }
     *sw_launches += *launches - before;
-    (void)n_pairs_ub;
     return VTX_OK;
 }
 
@@ -390,21 +472,21 @@ int grow_results(vtx_ctx* ctx, size_t need)
 {
     if (need <= ctx->res_cap) return VTX_OK;
     const size_t ncap = need + need / 4 + 1024;
-    DBuf* bufs[7] = { &ctx->r_row, &ctx->r_col, &ctx->r_ref, &ctx->r_alt, &ctx->r_unk, &ctx->r_val, &ctx->r_val2 };
-    const size_t esz[7] = { 4, 4, 4, 4, 4, 8, 8 };
-    for (int i = 0; i < 7; ++i) {
-        void* np = nullptr;
-        cudaError_t e = cudaMalloc(&np, ncap * esz[i]);
-        if (e != cudaSuccess) return set_err(ctx, VTX_E_NOMEM, "result cudaMalloc(%zu) failed: %s", ncap * esz[i], cudaGetErrorString(e));
-        if (bufs[i]->p && ctx->res_ub && !ctx->finished)
-            CK(cudaMemcpyAsync(np, bufs[i]->p, ctx->res_ub * esz[i], cudaMemcpyDeviceToDevice, ctx->stream));
-        if (bufs[i]->p) {
+    for (int i = 0; i < kResArrays; ++i) {
+        DBuf& b = ctx->res[i];
+        DBuf nb;
+        cudaError_t e = cudaMalloc(&nb.p, ncap * kResEsz[i]);
+        if (e != cudaSuccess) { nb.p = nullptr; return set_err(ctx, VTX_E_NOMEM, "result cudaMalloc(%zu) failed: %s", ncap * kResEsz[i], cudaGetErrorString(e)); }
+        nb.cap = ncap * kResEsz[i];
+        if (b.p && ctx->res_ub && !ctx->finished)
+            CK(cudaMemcpyAsync(nb.p, b.p, ctx->res_ub * kResEsz[i], cudaMemcpyDeviceToDevice, ctx->stream));
+        if (b.p) {
             CK(cudaStreamSynchronize(ctx->stream));
             if (ctx->fetch_stream) CK(cudaStreamSynchronize(ctx->fetch_stream));
             if (ctx->comm_stream) CK(cudaStreamSynchronize(ctx->comm_stream));
-            CK(cudaFree(bufs[i]->p));
+            CK(b.release());
         }
-        bufs[i]->p = np; bufs[i]->cap = ncap * esz[i];
+        b.swap(nb);
     }
     ctx->res_cap = ncap;
     return VTX_OK;
@@ -461,7 +543,7 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
     vtx_k_cand_filter<<<blocks_for(nc, 256), 256, 0, st>>>(nc, b.cand_read, P<int32_t>(ctx->read_col), b.read_umi, use_umi,
                                                            P<uint32_t>(ctx->keep), P<unsigned long long>(ctx->d_metrics));
     launches += 2;
-    rc = scan_u32(ctx, P<uint32_t>(ctx->keep), nc, P<uint32_t>(ctx->pidx), &launches);
+    rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->keep), nc, P<uint32_t>(ctx->pidx), &launches);
     if (rc) return rc;
     vtx_k_compact<<<blocks_for(nc, 256), 256, 0, st>>>(nc, b.cand_read, P<uint32_t>(ctx->keep), P<uint32_t>(ctx->pidx),
                                                        P<int32_t>(ctx->read_col), b.read_umi, use_umi, P<uint32_t>(ctx->pair_read),
@@ -511,14 +593,14 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
     vtx_k_finalize<<<blocks_for(nc, 256), 256, 0, st>>>(uint32_t(nc), n_pairs_ptr, ctx->cfg.mode, P<uint32_t>(ctx->cslot_col),
                                                         P<uint32_t>(ctx->ccnt), P<uint32_t>(ctx->keep2));
     ++launches;
-    rc = scan_u32(ctx, P<uint32_t>(ctx->keep2), nc, P<uint32_t>(ctx->oidx), &launches);
+    rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->keep2), nc, P<uint32_t>(ctx->oidx), &launches);
     if (rc) return rc;
     if (ctx->gather_guard) {       // a gather started after the previous finish may still be reading the local result arrays
         CK(cudaStreamWaitEvent(st, ctx->ev_gather, 0));
         ctx->gather_guard = false;
     }
-    ResultArrays out{ P<uint32_t>(ctx->r_row), P<uint32_t>(ctx->r_col), P<uint32_t>(ctx->r_ref), P<uint32_t>(ctx->r_alt),
-                      P<uint32_t>(ctx->r_unk), P<double>(ctx->r_val), P<double>(ctx->r_val2) };
+    ResultArrays out{ P<uint32_t>(ctx->res[0]), P<uint32_t>(ctx->res[1]), P<uint32_t>(ctx->res[2]), P<uint32_t>(ctx->res[3]),
+                      P<uint32_t>(ctx->res[4]), P<double>(ctx->res[5]), P<double>(ctx->res[6]) };
     vtx_k_emit<<<blocks_for(nc, 256), 256, 0, st>>>(uint32_t(nc), ctx->cfg.mode, P<uint32_t>(ctx->keep2), P<uint32_t>(ctx->oidx),
                                                     P<unsigned long long>(ctx->d_res_n), P<uint32_t>(ctx->cslot_col),
                                                     P<uint32_t>(ctx->cslot_locus), b.locus_row, P<uint32_t>(ctx->ccnt), out);
@@ -535,12 +617,12 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
     return VTX_OK;
 }
 
-// One view of a host batch for validation, whichever layout it arrived in.
-struct HostView {
+// One view of a batch, whichever layout it arrived in.  Building it reads no array, so it serves host and device batches.
+struct BatchView {
     uint32_t n_loci = 0, n_reads = 0; uint64_t n_cand = 0;
     const uint32_t *locus_row = nullptr, *ref_off = nullptr, *ref_len = nullptr, *alt_off = nullptr, *alt_len = nullptr;
     const uint64_t* cand_start = nullptr; const uint8_t* hap = nullptr; uint64_t hap_len = 0;
-    uint64_t nib_len = 0, cb_bytes_len = 0;
+    const uint8_t* read_nib = nullptr; uint64_t nib_len = 0; const uint8_t* cb_bytes = nullptr; uint64_t cb_bytes_len = 0;   // cb_bytes_len: vtx_batch
     const uint64_t* read_off = nullptr; const uint32_t* read_len = nullptr; const uint32_t* cb_off = nullptr; const uint16_t* cb_len = nullptr;   // vtx_batch
     const uint32_t* read_off4 = nullptr; const uint16_t* read_len16 = nullptr; const uint64_t* cb_key = nullptr;                                // vtx_batch2
     uint32_t n_exotic = 0; const uint32_t* cb_off_ex = nullptr;
@@ -548,30 +630,45 @@ struct HostView {
     bool v2 = false;
 };
 
-HostView view_of(const vtx_batch* b)
+BatchView view_of(const vtx_batch* b)
 {
-    HostView v;
+    BatchView v;
     v.n_loci = b->n_loci; v.n_reads = b->n_reads; v.n_cand = b->n_cand;
     v.locus_row = b->locus_row; v.ref_off = b->ref_off; v.ref_len = b->ref_len; v.alt_off = b->alt_off; v.alt_len = b->alt_len;
-    v.cand_start = b->cand_start; v.hap = b->hap_bytes; v.hap_len = b->hap_bytes_len; v.nib_len = b->read_nib_len; v.cb_bytes_len = b->cb_bytes_len;
+    v.cand_start = b->cand_start; v.hap = b->hap_bytes; v.hap_len = b->hap_bytes_len;
+    v.read_nib = b->read_nib; v.nib_len = b->read_nib_len; v.cb_bytes = b->cb_bytes; v.cb_bytes_len = b->cb_bytes_len;
     v.read_off = b->read_off; v.read_len = b->read_len; v.cb_off = b->read_cb_off; v.cb_len = b->read_cb_len;
     v.umi = b->read_umi_key; v.cand_read = b->cand_read;
     return v;
 }
-HostView view_of(const vtx_batch2* b)
+BatchView view_of(const vtx_batch2* b)
 {
-    HostView v;
+    BatchView v;
     v.v2 = true;
     v.n_loci = b->n_loci; v.n_reads = b->n_reads; v.n_cand = b->n_cand;
     v.locus_row = b->locus_row; v.ref_off = b->ref_off; v.ref_len = b->ref_len; v.alt_off = b->alt_off; v.alt_len = b->alt_len;
-    v.cand_start = b->cand_start; v.hap = b->hap_bytes; v.hap_len = b->hap_bytes_len; v.nib_len = b->read_nib_len;
+    v.cand_start = b->cand_start; v.hap = b->hap_bytes; v.hap_len = b->hap_bytes_len;
+    v.read_nib = b->read_nib; v.nib_len = b->read_nib_len; v.cb_bytes = b->cb_bytes;
     v.read_off4 = b->read_off4; v.read_len16 = b->read_len; v.cb_key = b->read_cb_key; v.n_exotic = b->n_exotic_cb; v.cb_off_ex = b->cb_off;
-    v.cb_bytes_len = (b->n_exotic_cb && b->cb_off) ? b->cb_off[b->n_exotic_cb] : 0;
     v.umi = b->read_umi_key; v.cand_read = b->cand_read;
     return v;
 }
 
-int validate_batch(vtx_ctx* ctx, const HostView& b, bool device)
+// the kernels' view of a batch whose arrays are on the device (the slim layout's read arrays come from expand_reads)
+DevBatch dev_batch_of(const BatchView& v, uint32_t max_read_len, uint32_t max_hap_len)
+{
+    DevBatch d{};
+    d.n_loci = v.n_loci; d.n_reads = v.n_reads; d.n_cand = v.n_cand;
+    d.locus_row = v.locus_row; d.hap = v.hap; d.ref_off = v.ref_off; d.ref_len = v.ref_len; d.alt_off = v.alt_off; d.alt_len = v.alt_len;
+    d.cand_start = v.cand_start; d.read_nib = v.read_nib; d.cb_bytes = v.cb_bytes;
+    d.read_off = v.read_off; d.read_len = v.read_len; d.read_cb_off = v.cb_off; d.read_cb_len = v.cb_len;
+    d.read_cb_key = v.cb_key; d.cb_off_ex = v.cb_off_ex;
+    d.read_umi = v.umi; d.cand_read = v.cand_read;
+    d.max_read_len = max_read_len; d.max_hap_len = max_hap_len;
+    return d;
+}
+
+int validate_batch(vtx_ctx* ctx, const BatchView& b)
 {
     if (b.n_cand >= 0xFFFFFFF0ull) return set_err(ctx, VTX_E_INVALID, "n_cand %llu exceeds 2^32 per shard; split the shard", (unsigned long long)b.n_cand);
     if (b.n_loci && (!b.locus_row || !b.ref_off || !b.ref_len || !b.alt_off || !b.alt_len || !b.cand_start))
@@ -584,7 +681,6 @@ int validate_batch(vtx_ctx* ctx, const HostView& b, bool device)
     if (b.n_cand && !b.cand_read && !(b.v2 && b.n_cand == b.n_reads)) return set_err(ctx, VTX_E_INVALID, "cand_read missing (NULL means identity and needs n_cand == n_reads in a vtx_batch2)");
     if (b.hap_len >= 0xFFFFFFFFull) return set_err(ctx, VTX_E_INVALID, "haplotype pool exceeds 4 GiB; split the shard");
     if (b.v2 && b.nib_len >= (uint64_t(1) << 34)) return set_err(ctx, VTX_E_INVALID, "read pool exceeds 16 GiB; split the shard");
-    (void)device;
     return VTX_OK;
 }
 
@@ -631,7 +727,7 @@ uint32_t class_mask_of(const bool* seen, bool allow_split, bool allow_multi, boo
 
 // host-side checks that need to touch the (host) arrays; also returns max lengths.  Runs on a few host
 // threads while the shard's H2D copies are already in flight (the kernels are only enqueued afterwards).
-int scan_host_batch(vtx_ctx* ctx, const HostView& b, uint32_t* max_read, uint32_t* max_hap, bool check_cands,
+int scan_host_batch(vtx_ctx* ctx, const BatchView& b, uint32_t* max_read, uint32_t* max_hap, bool check_cands,
                     uint64_t* max_depth = nullptr, bool* shapes_seen = nullptr)
 {
     if (check_cands && b.n_loci && (b.cand_start[0] != 0 || b.cand_start[b.n_loci] != b.n_cand))
@@ -747,22 +843,163 @@ int claim_slot(vtx_ctx* ctx, InSlot** out)
     return VTX_OK;
 }
 
-int upload_common(vtx_ctx* ctx, InSlot* sl, const vtx_batch* hb, DevBatch& d)
+// the locus arrays and the haplotype pool, both layouts
+int upload_loci(vtx_ctx* ctx, InSlot* sl, const BatchView& h, DevBatch& d)
 {
-    const uint32_t nl = hb->n_loci, nr = hb->n_reads;
-    UP(sl->locus_row, hb->locus_row, size_t(nl) * 4);
-    UP(sl->hap, hb->hap_bytes, hb->hap_bytes_len);
-    UP(sl->ref_off, hb->ref_off, size_t(nl) * 4); UP(sl->ref_len, hb->ref_len, size_t(nl) * 4);
-    UP(sl->alt_off, hb->alt_off, size_t(nl) * 4); UP(sl->alt_len, hb->alt_len, size_t(nl) * 4);
-    UP(sl->read_nib, hb->read_nib, hb->read_nib_len);
-    UP(sl->read_off, hb->read_off, size_t(nr) * 8); UP(sl->read_len, hb->read_len, size_t(nr) * 4);
-    d.n_loci = nl; d.n_reads = nr;
+    const size_t nl = h.n_loci;
+    UP(sl->locus_row, h.locus_row, nl * 4);
+    UP(sl->hap, h.hap, h.hap_len);
+    UP(sl->ref_off, h.ref_off, nl * 4); UP(sl->ref_len, h.ref_len, nl * 4);
+    UP(sl->alt_off, h.alt_off, nl * 4); UP(sl->alt_len, h.alt_len, nl * 4);
+    d.n_loci = h.n_loci; d.n_reads = h.n_reads; d.n_cand = h.n_cand;
     d.locus_row = P<uint32_t>(sl->locus_row); d.hap = P<uint8_t>(sl->hap);
     d.ref_off = P<uint32_t>(sl->ref_off); d.ref_len = P<uint32_t>(sl->ref_len);
     d.alt_off = P<uint32_t>(sl->alt_off); d.alt_len = P<uint32_t>(sl->alt_len);
+    return VTX_OK;
+}
+
+// loci and reads of a vtx_batch (what vtx_score_pairs needs)
+int upload_common(vtx_ctx* ctx, InSlot* sl, const BatchView& h, DevBatch& d)
+{
+    int rc = upload_loci(ctx, sl, h, d);
+    if (rc) return rc;
+    UP(sl->read_nib, h.read_nib, h.nib_len);
+    UP(sl->read_off, h.read_off, size_t(h.n_reads) * 8); UP(sl->read_len, h.read_len, size_t(h.n_reads) * 4);
     d.read_nib = P<uint8_t>(sl->read_nib); d.read_off = P<uint64_t>(sl->read_off); d.read_len = P<uint32_t>(sl->read_len);
     return VTX_OK;
 }
+
+// vtx_batch: the rest of the shard
+int upload_batch(vtx_ctx* ctx, InSlot* sl, const BatchView& h, DevBatch& d)
+{
+    int rc = upload_common(ctx, sl, h, d);
+    if (rc) return rc;
+    const size_t nr = h.n_reads;
+    UP(sl->cand_start, h.cand_start, size_t(h.n_loci + 1) * 8);
+    UP(sl->cb_bytes, h.cb_bytes, h.cb_bytes_len);
+    UP(sl->read_cb_off, h.cb_off, nr * 4); UP(sl->read_cb_len, h.cb_len, nr * 2);
+    if (h.umi) UP(sl->read_umi, h.umi, nr * 8);
+    UP(sl->cand_read, h.cand_read, size_t(h.n_cand) * 4);
+    d.cand_start = P<uint64_t>(sl->cand_start); d.cb_bytes = P<uint8_t>(sl->cb_bytes);
+    d.read_cb_off = P<uint32_t>(sl->read_cb_off); d.read_cb_len = P<uint16_t>(sl->read_cb_len);
+    d.read_umi = h.umi ? P<uint64_t>(sl->read_umi) : nullptr; d.cand_read = P<uint32_t>(sl->cand_read);
+    return VTX_OK;
+}
+
+// vtx_batch2: the slim arrays; the engine's read arrays are derived from them on the device (expand_reads)
+int upload_batch2(vtx_ctx* ctx, InSlot* sl, const BatchView& h, DevBatch& d)
+{
+    int rc = upload_loci(ctx, sl, h, d);
+    if (rc) return rc;
+    const size_t nr = h.n_reads;
+    UP(sl->cand_start, h.cand_start, size_t(h.n_loci + 1) * 8);
+    UP(sl->read_nib, h.read_nib, h.nib_len);
+    if (h.read_off4) UP(sl->read_off4, h.read_off4, nr * 4);
+    UP(sl->read_len16, h.read_len16, nr * 2);
+    UP(sl->read_cb_key, h.cb_key, nr * 8);
+    if (h.n_exotic) { UP(sl->cb_bytes, h.cb_bytes, h.cb_off_ex[h.n_exotic]); UP(sl->cb_off_ex, h.cb_off_ex, size_t(h.n_exotic + 1) * 4); }
+    if (h.umi) UP(sl->read_umi, h.umi, nr * 8);
+    if (h.cand_read) UP(sl->cand_read, h.cand_read, size_t(h.n_cand) * 4);
+    d.cand_start = P<uint64_t>(sl->cand_start); d.read_nib = P<uint8_t>(sl->read_nib);
+    d.read_cb_key = P<uint64_t>(sl->read_cb_key);
+    d.cb_bytes = h.n_exotic ? P<uint8_t>(sl->cb_bytes) : nullptr; d.cb_off_ex = h.n_exotic ? P<uint32_t>(sl->cb_off_ex) : nullptr;
+    d.read_umi = h.umi ? P<uint64_t>(sl->read_umi) : nullptr;
+    d.cand_read = h.cand_read ? P<uint32_t>(sl->cand_read) : nullptr;
+    return VTX_OK;
+}
+
+// slim read arrays (device) -> the engine's internal read_off (u64 bytes) / read_len (u32)
+int expand_reads(vtx_ctx* ctx, uint32_t nr, const uint16_t* d_len16, const uint32_t* d_off4, DevBatch& d)
+{
+    ENS(ctx->x_read_off, size_t(nr ? nr : 1) * 8); ENS(ctx->x_read_len, size_t(nr ? nr : 1) * 4);
+    if (nr) {
+        if (!d_off4) {          // dense pool: offsets are the running sum of the 4-byte units of the reads before
+            ENS(ctx->x_units, size_t(nr) * 4); ENS(ctx->x_off4, size_t(nr + 1) * 4);
+            vtx_k_read_units<<<blocks_for(nr, 256), 256, 0, ctx->stream>>>(nr, d_len16, P<uint32_t>(ctx->x_units));
+            int rc = scan_u32(ctx, ctx->stream, ctx->scan_sums, P<uint32_t>(ctx->x_units), nr, P<uint32_t>(ctx->x_off4), nullptr);
+            if (rc) return rc;
+            d_off4 = P<uint32_t>(ctx->x_off4);
+        }
+        vtx_k_expand_reads<<<blocks_for(nr, 256), 256, 0, ctx->stream>>>(nr, d_len16, d_off4, P<uint64_t>(ctx->x_read_off), P<uint32_t>(ctx->x_read_len));
+        CK(cudaGetLastError());
+    }
+    d.read_off = P<uint64_t>(ctx->x_read_off); d.read_len = P<uint32_t>(ctx->x_read_len);
+    return VTX_OK;
+}
+
+// Entry checks shared by the submits: barcodes set, batch present, the layout's own checks, the promised read length;
+// then the device is selected and the submit gets its timing record.
+template <typename Check>
+int begin_submit(vtx_ctx* ctx, const void* batch, const char* fn, const char* what, Check check, uint32_t max_read_len, TimeRec** tr)
+{
+    if (!ctx->have_barcodes) return set_err(ctx, VTX_E_STATE, "vtx_set_barcodes must be called before %s", fn);
+    if (!batch) return set_err(ctx, VTX_E_INVALID, "%s is NULL", what);
+    int rc = check();
+    if (rc) return rc;
+    if (max_read_len > uint32_t(kMaxRead)) return set_err(ctx, VTX_E_UNSUPPORTED, "reads longer than %d bases are not supported", kMaxRead);
+    CK(cudaSetDevice(ctx->device));
+    *tr = new_trec(ctx);
+    if (!*tr) return set_err(ctx, VTX_E_CUDA, "cudaEventCreate failed");
+    return VTX_OK;
+}
+
+// vtx_submit / vtx_submit2: a host batch of either layout
+template <typename Batch>
+int submit_host(vtx_ctx* ctx, const Batch* hb, const char* fn)
+{
+    Nvtx nvtx_range(fn);
+    BatchView h;
+    TimeRec* tr = nullptr;
+    int rc = begin_submit(ctx, hb, fn, "batch", [&] { h = view_of(hb); return validate_batch(ctx, h); }, 0, &tr);
+    if (rc) return rc;
+    InSlot* sl = nullptr;
+    rc = claim_slot(ctx, &sl);
+    if (rc) return rc;
+    // 1. start the copies of this shard on the copy stream (they overlap the previous shard's kernels) ...
+    DevBatch d{};
+    CK(cudaEventRecord(tr->ev[EV_START], ctx->copy_stream));
+    rc = h.v2 ? upload_batch2(ctx, sl, h, d) : upload_batch(ctx, sl, h, d);
+    if (rc) return rc;
+    CK(cudaEventRecord(tr->ev[EV_H2D], ctx->copy_stream));
+    CK(cudaEventRecord(sl->copy_done, ctx->copy_stream));
+    tr->had_h2d = true;
+    // 2. ... validate the host arrays meanwhile; nothing has been launched on them yet
+    bool shapes[kNumShapes] = {};
+    { Nvtx r_val("vtx: validate host batch (copies in flight)");
+      rc = scan_host_batch(ctx, h, &d.max_read_len, &d.max_hap_len, true, &d.max_depth, shapes); }
+    if (rc) { cudaStreamSynchronize(ctx->copy_stream); --ctx->trec_used; return rc; }
+    d.class_mask = host_class_mask(ctx, shapes, d.max_read_len, d.max_hap_len);
+    // 3. kernels wait for the copy, and release the slot when done
+    CK(cudaStreamWaitEvent(ctx->stream, sl->copy_done, 0));
+    CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));
+    if (h.v2) {
+        rc = expand_reads(ctx, h.n_reads, P<uint16_t>(sl->read_len16), h.read_off4 ? P<uint32_t>(sl->read_off4) : nullptr, d);
+        if (rc) return rc;
+    }
+    rc = process_batch(ctx, d, tr);
+    if (rc) return rc;
+    CK(cudaEventRecord(sl->free_ev, ctx->stream));
+    return VTX_OK;
+}
+
+// vtx_submit_device_ex / vtx_submit2_device: the batch's arrays are already on the device
+template <typename Batch>
+int submit_resident(vtx_ctx* ctx, const Batch* db, const char* fn, uint32_t max_read_len, uint32_t max_hap_len)
+{
+    BatchView v;
+    TimeRec* tr = nullptr;
+    int rc = begin_submit(ctx, db, fn, "batch", [&] { v = view_of(db); return validate_batch(ctx, v); }, max_read_len, &tr);
+    if (rc) return rc;
+    DevBatch d = dev_batch_of(v, max_read_len, max_hap_len);
+    CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));
+    if (v.v2) {
+        rc = expand_reads(ctx, v.n_reads, v.read_len16, v.read_off4, d);
+        if (rc) return rc;
+    }
+    return process_batch(ctx, d, tr);
+}
+
+void comm_destroy(vtx_ctx* ctx);      // with the NCCL loader below
 
 }  // namespace
 
@@ -813,15 +1050,15 @@ int vtx_create(const vtx_config* cfg, vtx_ctx** out)
     pe = cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking);
     if (pe != cudaSuccess) { g_create_error = cudaGetErrorString(pe); vtx_destroy(ctx); return VTX_E_CUDA; }
     cudaStreamCreateWithFlags(&ctx->fetch_stream, cudaStreamNonBlocking);
-    if (cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_cum), kMaxCum * 8, cudaHostAllocMapped) == cudaSuccess) {
-        if (cudaHostGetDevicePointer(reinterpret_cast<void**>(&ctx->d_cum), ctx->h_cum, 0) != cudaSuccess) ctx->d_cum = nullptr;
-    } else { ctx->h_cum = nullptr; cudaGetLastError(); }
+    if (ctx->h_cum.alloc(kMaxCum * 8, cudaHostAllocMapped) == cudaSuccess) {
+        if (cudaHostGetDevicePointer(reinterpret_cast<void**>(&ctx->d_cum), ctx->h_cum.p, 0) != cudaSuccess) ctx->d_cum = nullptr;
+    } else cudaGetLastError();
     for (auto& sl : ctx->slot) {
         cudaEventCreateWithFlags(&sl.copy_done, cudaEventDisableTiming);
         cudaEventCreateWithFlags(&sl.free_ev, cudaEventDisableTiming);
     }
     bool ok = cudaMalloc(&ctx->d_metrics.p, 64) == cudaSuccess && cudaMalloc(&ctx->d_res_n.p, 64) == cudaSuccess &&
-              cudaHostAlloc(&ctx->h_scalars, 64, cudaHostAllocDefault) == cudaSuccess;
+              ctx->h_scalars.alloc(64) == cudaSuccess;
     if (!ok) { g_create_error = "allocation of context scalars failed"; vtx_destroy(ctx); return VTX_E_NOMEM; }
     ctx->d_metrics.cap = 64; ctx->d_res_n.cap = 64;
     cudaMemsetAsync(ctx->d_metrics.p, 0, 64, ctx->stream);
@@ -830,57 +1067,22 @@ int vtx_create(const vtx_config* cfg, vtx_ctx** out)
     return VTX_OK;
 }
 
-void vtx_comm_destroy_internal(vtx_ctx* ctx);   // vtx_comm.cpp
-
 void vtx_destroy(vtx_ctx* ctx)
 {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    if (ctx->comm_stream) cudaStreamSynchronize(ctx->comm_stream);
-    vtx_comm_destroy_internal(ctx);
-    if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
-    for (auto& sl : ctx->slot) {
-        DBuf* sb[] = { &sl.locus_row, &sl.hap, &sl.ref_off, &sl.ref_len, &sl.alt_off, &sl.alt_len, &sl.cand_start, &sl.read_nib,
-                       &sl.read_off, &sl.read_len, &sl.cb_bytes, &sl.read_cb_off, &sl.read_cb_len, &sl.read_umi, &sl.cand_read,
-                       &sl.read_off4, &sl.read_len16, &sl.read_cb_key, &sl.cb_off_ex };
-        for (DBuf* b : sb) if (b->p) cudaFree(b->p);
-        if (sl.copy_done) cudaEventDestroy(sl.copy_done);
-        if (sl.free_ev) cudaEventDestroy(sl.free_ev);
-    }
-    DBuf* all[] = { &ctx->bc_slot, &ctx->bc_bytes, &ctx->bc_off, &ctx->bck_key, &ctx->bck_idx, &ctx->x_read_off, &ctx->x_read_len,
-                    &ctx->x_units, &ctx->x_off4, &ctx->band_scratch, &ctx->inf_comp, &ctx->inf_out, &ctx->inf_desc, &ctx->inf_status, &ctx->read_col,
-                    &ctx->keep, &ctx->pidx, &ctx->scan_sums, &ctx->pair_read, &ctx->pair_col, &ctx->pair_umi, &ctx->pair_locus,
-                    &ctx->pair_start, &ctx->tcount, &ctx->tstart, &ctx->pair_first, &ctx->pair_cslot, &ctx->pair_uslot, &ctx->cslot_col,
-                    &ctx->cslot_locus, &ctx->uslot_cslot, &ctx->ccnt, &ctx->ucnt, &ctx->keep2, &ctx->oidx, &ctx->tile_counters,
-                    &ctx->scratch, &ctx->pair_scores, &ctx->big_list, &ctx->slot_scratch, &ctx->d_metrics, &ctx->d_res_n, &ctx->r_row, &ctx->r_col, &ctx->r_ref,
-                    &ctx->r_alt, &ctx->r_unk, &ctx->r_val, &ctx->r_val2, &ctx->g_counts };
-    for (DBuf* b : all) if (b->p) cudaFree(b->p);
-    for (auto& b : ctx->g_dev) if (b.p) cudaFree(b.p);
-    if (ctx->stage_stream) { cudaStreamSynchronize(ctx->stage_stream); cudaStreamDestroy(ctx->stage_stream); }
-    for (auto& ss : ctx->sslot) {
-        DBuf* sb[] = { &ss.comp, &ss.desc, &ss.status, &ss.stream, &ss.entry, &ss.seg_count, &ss.seg_first, &ss.rec_off, &ss.rec_tid, &ss.rec_pos, &ss.rec_end,
-                       &ss.rec_fm, &ss.l_start, &ss.l_end, &ss.locus_row, &ss.hap, &ss.ref_off, &ss.ref_len, &ss.alt_off, &ss.alt_len, &ss.cand_count,
-                       &ss.cand_first, &ss.cand_rec, &ss.used, &ss.read_off, &ss.read_len, &ss.read_cb_off, &ss.read_cb_len, &ss.read_umi, &ss.cand_start, &ss.scalars };
-        for (DBuf* b : sb) if (b->p) cudaFree(b->p);
-        if (ss.staged) cudaEventDestroy(ss.staged);
-        if (ss.free_ev) cudaEventDestroy(ss.free_ev);
-    }
-    if (ctx->bam_metrics.p) cudaFree(ctx->bam_metrics.p);
-    if (ctx->stage_sums.p) cudaFree(ctx->stage_sums.p);
-    if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-    for (void* h : ctx->h_res) if (h) cudaFreeHost(h);
-    for (void* h : ctx->g_host) if (h) cudaFreeHost(h);
-    if (ctx->h_scalars) cudaFreeHost(ctx->h_scalars);
+    for (cudaStream_t s : { ctx->stream, ctx->comm_stream, ctx->copy_stream, ctx->stage_stream, ctx->fetch_stream })
+        if (s) cudaStreamSynchronize(s);
+    comm_destroy(ctx);
+    for (auto& sl : ctx->slot)
+        for (cudaEvent_t e : { sl.copy_done, sl.free_ev }) if (e) cudaEventDestroy(e);
+    for (auto& ss : ctx->sslot)
+        for (cudaEvent_t e : { ss.staged, ss.free_ev }) if (e) cudaEventDestroy(e);
     for (auto& tr : ctx->trecs) for (auto& ev : tr.ev) if (ev) cudaEventDestroy(ev);
-    if (ctx->comm_stream) { cudaStreamSynchronize(ctx->comm_stream); cudaStreamDestroy(ctx->comm_stream); }
     for (cudaEvent_t e : { ctx->ev_counts, ctx->ev_gather, ctx->ev_results }) if (e) cudaEventDestroy(e);
-    if (ctx->h_counts) cudaFreeHost(ctx->h_counts);
-    if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-    if (ctx->fetch_stream) cudaStreamDestroy(ctx->fetch_stream);
-    if (ctx->h_cum) cudaFreeHost(ctx->h_cum);
+    for (cudaStream_t s : { ctx->stage_stream, ctx->comm_stream, ctx->copy_stream, ctx->fetch_stream }) if (s) cudaStreamDestroy(s);
     if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;     // frees the device and pinned buffers it owns
 }
 
 int vtx_host_alloc(void** out, uint64_t bytes)
@@ -938,74 +1140,14 @@ int vtx_set_barcodes(vtx_ctx* ctx, const uint8_t* bytes, const uint32_t* off, ui
 
 int vtx_submit(vtx_ctx* ctx, const vtx_batch* hb)
 {
-    Nvtx nvtx_range("vtx_submit");
     if (!ctx) return VTX_E_INVALID;
-    if (!ctx->have_barcodes) return set_err(ctx, VTX_E_STATE, "vtx_set_barcodes must be called before vtx_submit");
-    if (!hb) return set_err(ctx, VTX_E_INVALID, "batch is NULL");
-    const HostView hv = view_of(hb);
-    int rc = validate_batch(ctx, hv, false);
-    if (rc) return rc;
-    CK(cudaSetDevice(ctx->device));
-    TimeRec* tr = new_trec(ctx);
-    if (!tr) return set_err(ctx, VTX_E_CUDA, "cudaEventCreate failed");
-    InSlot* sl = nullptr;
-    rc = claim_slot(ctx, &sl);
-    if (rc) return rc;
-    // 1. start the copies of this shard on the copy stream (they overlap the previous shard's kernels) ...
-    DevBatch d{};
-    CK(cudaEventRecord(tr->ev[EV_START], ctx->copy_stream));
-    rc = upload_common(ctx, sl, hb, d);
-    if (rc) return rc;
-    const uint32_t nl = hb->n_loci, nr = hb->n_reads;
-    UP(sl->cand_start, hb->cand_start, size_t(nl + 1) * 8);
-    UP(sl->cb_bytes, hb->cb_bytes, hb->cb_bytes_len);
-    UP(sl->read_cb_off, hb->read_cb_off, size_t(nr) * 4); UP(sl->read_cb_len, hb->read_cb_len, size_t(nr) * 2);
-    if (hb->read_umi_key) UP(sl->read_umi, hb->read_umi_key, size_t(nr) * 8);
-    UP(sl->cand_read, hb->cand_read, size_t(hb->n_cand) * 4);
-    CK(cudaEventRecord(tr->ev[EV_H2D], ctx->copy_stream));
-    CK(cudaEventRecord(sl->copy_done, ctx->copy_stream));
-    tr->had_h2d = true;
-    d.n_cand = hb->n_cand;
-    d.cand_start = P<uint64_t>(sl->cand_start); d.cb_bytes = P<uint8_t>(sl->cb_bytes);
-    d.read_cb_off = P<uint32_t>(sl->read_cb_off); d.read_cb_len = P<uint16_t>(sl->read_cb_len);
-    d.read_umi = hb->read_umi_key ? P<uint64_t>(sl->read_umi) : nullptr; d.cand_read = P<uint32_t>(sl->cand_read);
-    // 2. ... validate the host arrays meanwhile; nothing has been launched on them yet
-    bool shapes[kNumShapes] = {};
-    { Nvtx r_val("vtx: validate host batch (copies in flight)");
-      rc = scan_host_batch(ctx, hv, &d.max_read_len, &d.max_hap_len, true, &d.max_depth, shapes); }
-    if (rc) { cudaStreamSynchronize(ctx->copy_stream); --ctx->trec_used; return rc; }
-    d.class_mask = host_class_mask(ctx, shapes, d.max_read_len, d.max_hap_len);
-    // 3. kernels wait for the copy, and release the slot when done
-    CK(cudaStreamWaitEvent(ctx->stream, sl->copy_done, 0));
-    CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));
-    rc = process_batch(ctx, d, tr);
-    if (rc) return rc;
-    CK(cudaEventRecord(sl->free_ev, ctx->stream));
-    return VTX_OK;
+    return submit_host(ctx, hb, "vtx_submit");
 }
 
-// device batches carry their own bounds in the (otherwise unused) *_len fields of the pools:
-// the caller must pass max read / haplotype lengths through vtx_submit_device_ex.
 int vtx_submit_device_ex(vtx_ctx* ctx, const vtx_batch* db, uint32_t max_read_len, uint32_t max_hap_len)
 {
     if (!ctx) return VTX_E_INVALID;
-    if (!ctx->have_barcodes) return set_err(ctx, VTX_E_STATE, "vtx_set_barcodes must be called before vtx_submit_device");
-    if (!db) return set_err(ctx, VTX_E_INVALID, "batch is NULL");
-    int rc = validate_batch(ctx, view_of(db), true);
-    if (rc) return rc;
-    if (max_read_len > uint32_t(kMaxRead)) return set_err(ctx, VTX_E_UNSUPPORTED, "reads longer than %d bases are not supported", kMaxRead);
-    CK(cudaSetDevice(ctx->device));
-    DevBatch d{};
-    d.n_loci = db->n_loci; d.n_reads = db->n_reads; d.n_cand = db->n_cand;
-    d.locus_row = db->locus_row; d.hap = db->hap_bytes; d.ref_off = db->ref_off; d.ref_len = db->ref_len;
-    d.alt_off = db->alt_off; d.alt_len = db->alt_len; d.cand_start = db->cand_start; d.read_nib = db->read_nib;
-    d.read_off = db->read_off; d.read_len = db->read_len; d.cb_bytes = db->cb_bytes; d.read_cb_off = db->read_cb_off;
-    d.read_cb_len = db->read_cb_len; d.read_umi = db->read_umi_key; d.cand_read = db->cand_read;
-    d.max_read_len = max_read_len; d.max_hap_len = max_hap_len;
-    TimeRec* tr = new_trec(ctx);
-    if (!tr) return set_err(ctx, VTX_E_CUDA, "cudaEventCreate failed");
-    CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));
-    return process_batch(ctx, d, tr);
+    return submit_resident(ctx, db, "vtx_submit_device", max_read_len, max_hap_len);
 }
 
 int vtx_submit_device(vtx_ctx* ctx, const vtx_batch* db)
@@ -1015,121 +1157,17 @@ int vtx_submit_device(vtx_ctx* ctx, const vtx_batch* db)
     return vtx_submit_device_ex(ctx, db, kFastMaxRead, class_max_n(kNumFastClasses - 1));
 }
 
-// ---- slim layout -------------------------------------------------------------------------------------------------
-namespace {
-// slim read arrays (device) -> the engine's internal read_off (u64 bytes) / read_len (u32)
-int expand_reads(vtx_ctx* ctx, uint32_t nr, const uint16_t* d_len16, const uint32_t* d_off4, DevBatch& d, uint64_t* launches_unused = nullptr)
-{
-    (void)launches_unused;
-    ENS(ctx->x_read_off, size_t(nr ? nr : 1) * 8); ENS(ctx->x_read_len, size_t(nr ? nr : 1) * 4);
-    if (nr) {
-        if (!d_off4) {          // dense pool: offsets are the running sum of the 4-byte units of the reads before
-            ENS(ctx->x_units, size_t(nr) * 4); ENS(ctx->x_off4, size_t(nr + 1) * 4);
-            vtx_k_read_units<<<blocks_for(nr, 256), 256, 0, ctx->stream>>>(nr, d_len16, P<uint32_t>(ctx->x_units));
-            int rc = scan_u32(ctx, P<uint32_t>(ctx->x_units), nr, P<uint32_t>(ctx->x_off4), nullptr);
-            if (rc) return rc;
-            d_off4 = P<uint32_t>(ctx->x_off4);
-        }
-        vtx_k_expand_reads<<<blocks_for(nr, 256), 256, 0, ctx->stream>>>(nr, d_len16, d_off4, P<uint64_t>(ctx->x_read_off), P<uint32_t>(ctx->x_read_len));
-        CK(cudaGetLastError());
-    }
-    d.read_off = P<uint64_t>(ctx->x_read_off); d.read_len = P<uint32_t>(ctx->x_read_len);
-    return VTX_OK;
-}
-}  // namespace
-
 int vtx_submit2(vtx_ctx* ctx, const vtx_batch2* hb)
 {
-    Nvtx nvtx_range("vtx_submit2");
     if (!ctx) return VTX_E_INVALID;
-    if (!ctx->have_barcodes) return set_err(ctx, VTX_E_STATE, "vtx_set_barcodes must be called before vtx_submit2");
-    if (!hb) return set_err(ctx, VTX_E_INVALID, "batch is NULL");
-    const HostView hv = view_of(hb);
-    int rc = validate_batch(ctx, hv, false);
-    if (rc) return rc;
-    CK(cudaSetDevice(ctx->device));
-    TimeRec* tr = new_trec(ctx);
-    if (!tr) return set_err(ctx, VTX_E_CUDA, "cudaEventCreate failed");
-    InSlot* sl = nullptr;
-    rc = claim_slot(ctx, &sl);
-    if (rc) return rc;
-    DevBatch d{};
-    const uint32_t nl = hb->n_loci, nr = hb->n_reads;
-    CK(cudaEventRecord(tr->ev[EV_START], ctx->copy_stream));
-    UP(sl->locus_row, hb->locus_row, size_t(nl) * 4);
-    UP(sl->hap, hb->hap_bytes, hb->hap_bytes_len);
-    UP(sl->ref_off, hb->ref_off, size_t(nl) * 4); UP(sl->ref_len, hb->ref_len, size_t(nl) * 4);
-    UP(sl->alt_off, hb->alt_off, size_t(nl) * 4); UP(sl->alt_len, hb->alt_len, size_t(nl) * 4);
-    UP(sl->cand_start, hb->cand_start, size_t(nl + 1) * 8);
-    UP(sl->read_nib, hb->read_nib, hb->read_nib_len);
-    if (hb->read_off4) UP(sl->read_off4, hb->read_off4, size_t(nr) * 4);
-    UP(sl->read_len16, hb->read_len, size_t(nr) * 2);
-    UP(sl->read_cb_key, hb->read_cb_key, size_t(nr) * 8);
-    if (hb->n_exotic_cb) { UP(sl->cb_bytes, hb->cb_bytes, hv.cb_bytes_len); UP(sl->cb_off_ex, hb->cb_off, size_t(hb->n_exotic_cb + 1) * 4); }
-    if (hb->read_umi_key) UP(sl->read_umi, hb->read_umi_key, size_t(nr) * 8);
-    if (hb->cand_read) UP(sl->cand_read, hb->cand_read, size_t(hb->n_cand) * 4);
-    CK(cudaEventRecord(tr->ev[EV_H2D], ctx->copy_stream));
-    CK(cudaEventRecord(sl->copy_done, ctx->copy_stream));
-    tr->had_h2d = true;
-    d.n_loci = nl; d.n_reads = nr; d.n_cand = hb->n_cand;
-    d.locus_row = P<uint32_t>(sl->locus_row); d.hap = P<uint8_t>(sl->hap);
-    d.ref_off = P<uint32_t>(sl->ref_off); d.ref_len = P<uint32_t>(sl->ref_len);
-    d.alt_off = P<uint32_t>(sl->alt_off); d.alt_len = P<uint32_t>(sl->alt_len);
-    d.cand_start = P<uint64_t>(sl->cand_start); d.read_nib = P<uint8_t>(sl->read_nib);
-    d.read_cb_key = P<uint64_t>(sl->read_cb_key);
-    d.cb_bytes = hb->n_exotic_cb ? P<uint8_t>(sl->cb_bytes) : nullptr; d.cb_off_ex = hb->n_exotic_cb ? P<uint32_t>(sl->cb_off_ex) : nullptr;
-    d.read_cb_off = nullptr; d.read_cb_len = nullptr;
-    d.read_umi = hb->read_umi_key ? P<uint64_t>(sl->read_umi) : nullptr;
-    d.cand_read = hb->cand_read ? P<uint32_t>(sl->cand_read) : nullptr;
-    bool shapes[kNumShapes] = {};
-    { Nvtx r_val("vtx: validate host batch (copies in flight)");
-      rc = scan_host_batch(ctx, hv, &d.max_read_len, &d.max_hap_len, true, &d.max_depth, shapes); }
-    if (rc) { cudaStreamSynchronize(ctx->copy_stream); --ctx->trec_used; return rc; }
-    d.class_mask = host_class_mask(ctx, shapes, d.max_read_len, d.max_hap_len);
-    CK(cudaStreamWaitEvent(ctx->stream, sl->copy_done, 0));
-    CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));
-    rc = expand_reads(ctx, nr, P<uint16_t>(sl->read_len16), hb->read_off4 ? P<uint32_t>(sl->read_off4) : nullptr, d);
-    if (rc) return rc;
-    rc = process_batch(ctx, d, tr);
-    if (rc) return rc;
-    CK(cudaEventRecord(sl->free_ev, ctx->stream));
-    return VTX_OK;
+    return submit_host(ctx, hb, "vtx_submit2");
 }
 
 int vtx_submit2_device(vtx_ctx* ctx, const vtx_batch2* db, uint32_t max_read_len, uint32_t max_hap_len)
 {
     if (!ctx) return VTX_E_INVALID;
-    if (!ctx->have_barcodes) return set_err(ctx, VTX_E_STATE, "vtx_set_barcodes must be called before vtx_submit2_device");
-    if (!db) return set_err(ctx, VTX_E_INVALID, "batch is NULL");
-    HostView hv = view_of(db); hv.cb_bytes_len = 0;       // device pointers: nothing may be dereferenced here
-    hv.cb_off_ex = db->cb_off;
-    int rc = validate_batch(ctx, hv, true);
-    if (rc) return rc;
-    if (max_read_len > uint32_t(kMaxRead)) return set_err(ctx, VTX_E_UNSUPPORTED, "reads longer than %d bases are not supported", kMaxRead);
-    CK(cudaSetDevice(ctx->device));
-    DevBatch d{};
-    d.n_loci = db->n_loci; d.n_reads = db->n_reads; d.n_cand = db->n_cand;
-    d.locus_row = db->locus_row; d.hap = db->hap_bytes; d.ref_off = db->ref_off; d.ref_len = db->ref_len;
-    d.alt_off = db->alt_off; d.alt_len = db->alt_len; d.cand_start = db->cand_start; d.read_nib = db->read_nib;
-    d.read_cb_key = db->read_cb_key; d.cb_bytes = db->cb_bytes; d.cb_off_ex = db->cb_off; d.read_cb_off = nullptr; d.read_cb_len = nullptr;
-    d.read_umi = db->read_umi_key; d.cand_read = db->cand_read;
-    d.max_read_len = max_read_len; d.max_hap_len = max_hap_len;
-    TimeRec* tr = new_trec(ctx);
-    if (!tr) return set_err(ctx, VTX_E_CUDA, "cudaEventCreate failed");
-    CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));
-    rc = expand_reads(ctx, db->n_reads, db->read_len, db->read_off4, d);
-    if (rc) return rc;
-    return process_batch(ctx, d, tr);
+    return submit_resident(ctx, db, "vtx_submit2_device", max_read_len, max_hap_len);
 }
-
-static int inflate_attr(vtx_ctx* ctx)        // the inflate kernel's tables + input windows need the opt-in shared-memory size
-{
-    if (ctx->inflate_attr_set) return VTX_OK;
-    CK(cudaFuncSetAttribute(inflate::vtx_k_bgzf_inflate, cudaFuncAttributeMaxDynamicSharedMemorySize, int(inflate::inflate_smem_bytes())));
-    ctx->inflate_attr_set = true;
-    return VTX_OK;
-}
-
 int vtx_bgzf_inflate(vtx_ctx* ctx, const vtx_bgzf_block* blocks, uint32_t n_blocks, const uint8_t* comp, uint64_t comp_len,
                      uint8_t* out, uint64_t out_len, int32_t* status, uint32_t flags)
 {
@@ -1153,12 +1191,8 @@ int vtx_bgzf_inflate(vtx_ctx* ctx, const vtx_bgzf_block* blocks, uint32_t n_bloc
     CK(cudaMemcpyAsync(ctx->inf_comp.p, comp, comp_len, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->inf_desc.p, blocks, size_t(n_blocks) * sizeof(vtx_bgzf_block), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(ctx->tile_counters.p, 0, 64, st));
-    const unsigned ctas = unsigned(std::min<uint64_t>((n_blocks + inflate::kInflateWarps - 1) / inflate::kInflateWarps, uint64_t(ctx->n_sm) * 6));
-    if (int rc_attr = inflate_attr(ctx)) return rc_attr;
-    inflate::vtx_k_bgzf_inflate<<<ctas, inflate::kInflateWarps * 32, inflate::inflate_smem_bytes(), st>>>(
-        P<inflate::BlockDesc>(ctx->inf_desc), n_blocks, P<uint8_t>(ctx->inf_comp), P<uint8_t>(ctx->inf_out), P<int32_t>(ctx->inf_status),
-        P<uint32_t>(ctx->tile_counters), (flags & VTX_BGZF_CHECK_CRC) ? 1 : 0);
-    CK(cudaGetLastError());
+    if (int rc = launch_inflate(ctx, st, ctx->inf_desc.p, n_blocks, ctx->inf_comp.p, ctx->inf_out.p, ctx->inf_status.p,
+                                P<uint32_t>(ctx->tile_counters), (flags & VTX_BGZF_CHECK_CRC) ? 1 : 0)) return rc;
     if (out_len) CK(cudaMemcpyAsync(out, ctx->inf_out.p, out_len, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(status, ctx->inf_status.p, size_t(n_blocks) * 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1170,64 +1204,52 @@ int vtx_bgzf_inflate(vtx_ctx* ctx, const vtx_bgzf_block* blocks, uint32_t n_bloc
 // -------------------------------------------------------------------------------------------------
 // vtx_submit_bam: inflate + record scan + fetch + filters + tags on the device (vtx_inflate.cuh, vtx_stage.cuh)
 // -------------------------------------------------------------------------------------------------
-namespace {
-int scan_u32_on(vtx_ctx* ctx, cudaStream_t st, const uint32_t* in, uint64_t n, uint32_t* out, DBuf& sums)
-{
-    const unsigned nb = std::max(1u, blocks_for(n, kScanTile));
-    int rc = ensure(ctx, sums, size_t(nb) * 4);
-    if (rc) return rc;
-    vtx_k_scan_tiles<<<nb, kScanThreads, 0, st>>>(in, n, out, P<uint32_t>(sums));
-    vtx_k_scan_sums<<<1, kScanThreads, 0, st>>>(P<uint32_t>(sums), nb, out + n);
-    vtx_k_scan_add<<<nb, kScanThreads, 0, st>>>(out, n, P<uint32_t>(sums));
-    CK(cudaGetLastError());
-    return VTX_OK;
-}
-}  // namespace
 
 int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
 {
     if (!ctx) return VTX_E_INVALID;
     Nvtx nvtx_range("vtx_submit_bam");
-    if (!ctx->have_barcodes) return set_err(ctx, VTX_E_STATE, "vtx_set_barcodes must be called before vtx_submit_bam");
-    if (!sh) return set_err(ctx, VTX_E_INVALID, "shard is NULL");
-    const uint32_t nl = sh->n_loci, nm = sh->n_members, ne = sh->n_entry;
-    if (nl && (!sh->locus_row || !sh->locus_start || !sh->locus_end || !sh->ref_off || !sh->ref_len || !sh->alt_off || !sh->alt_len))
-        return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: locus arrays missing");
-    if (nm && (!sh->members || !sh->comp)) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: members missing");
-    if ((ne == 1) || (ne && !sh->entry_off)) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: entry_off needs at least a start and an end");
-    if (sh->hap_bytes_len >= 0xFFFFFFFFull) return set_err(ctx, VTX_E_INVALID, "haplotype pool exceeds 4 GiB; split the shard");
+    uint32_t nl = 0, nm = 0, ne = 0, max_hap = 0;
     uint64_t stream_len = 0;
-    uint32_t max_hap = 0;
-    for (uint32_t i = 0; i < nm; ++i) {
-        const vtx_bgzf_block& b = sh->members[i];
-        if ((b.in_off & 3) || b.in_off + b.in_len > sh->comp_len || b.out_len > 65536u || b.out_off != stream_len)
-            return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: member %u: payload on a 4-byte boundary inside comp, out_off = running sum of out_len", i);
-        stream_len += b.out_len;
-    }
-    if (stream_len >= 0xFFFFFFFFull) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: more than 4 GiB of records in one shard; split the shard");
-    for (uint32_t i = 0; i < ne; ++i)
-        if (sh->entry_off[i] > stream_len || (i && sh->entry_off[i] <= sh->entry_off[i - 1])) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: entry_off must ascend inside the stream");
-    for (uint32_t l = 0; l < nl; ++l) {
-        if ((sh->ref_off[l] & 15) || (sh->alt_off[l] & 15) || uint64_t(sh->ref_off[l]) + sh->ref_len[l] > sh->hap_bytes_len ||
-            uint64_t(sh->alt_off[l]) + sh->alt_len[l] > sh->hap_bytes_len) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: locus %u: bad haplotype window", l);
-        if (l && (sh->locus_row[l] <= sh->locus_row[l - 1])) return set_err(ctx, VTX_E_INVALID, "locus_row must be strictly ascending (locus %u)", l);
-        max_hap = std::max(max_hap, std::max(sh->ref_len[l], sh->alt_len[l]));
-    }
-    CK(cudaSetDevice(ctx->device));
+    auto check = [&]() -> int {
+        nl = sh->n_loci; nm = sh->n_members; ne = sh->n_entry;
+        if (nl && (!sh->locus_row || !sh->locus_start || !sh->locus_end || !sh->ref_off || !sh->ref_len || !sh->alt_off || !sh->alt_len))
+            return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: locus arrays missing");
+        if (nm && (!sh->members || !sh->comp)) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: members missing");
+        if ((ne == 1) || (ne && !sh->entry_off)) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: entry_off needs at least a start and an end");
+        if (sh->hap_bytes_len >= 0xFFFFFFFFull) return set_err(ctx, VTX_E_INVALID, "haplotype pool exceeds 4 GiB; split the shard");
+        for (uint32_t i = 0; i < nm; ++i) {
+            const vtx_bgzf_block& b = sh->members[i];
+            if ((b.in_off & 3) || b.in_off + b.in_len > sh->comp_len || b.out_len > 65536u || b.out_off != stream_len)
+                return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: member %u: payload on a 4-byte boundary inside comp, out_off = running sum of out_len", i);
+            stream_len += b.out_len;
+        }
+        if (stream_len >= 0xFFFFFFFFull) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: more than 4 GiB of records in one shard; split the shard");
+        for (uint32_t i = 0; i < ne; ++i)
+            if (sh->entry_off[i] > stream_len || (i && sh->entry_off[i] <= sh->entry_off[i - 1])) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: entry_off must ascend inside the stream");
+        for (uint32_t l = 0; l < nl; ++l) {
+            if ((sh->ref_off[l] & 15) || (sh->alt_off[l] & 15) || uint64_t(sh->ref_off[l]) + sh->ref_len[l] > sh->hap_bytes_len ||
+                uint64_t(sh->alt_off[l]) + sh->alt_len[l] > sh->hap_bytes_len) return set_err(ctx, VTX_E_INVALID, "vtx_submit_bam: locus %u: bad haplotype window", l);
+            if (l && (sh->locus_row[l] <= sh->locus_row[l - 1])) return set_err(ctx, VTX_E_INVALID, "locus_row must be strictly ascending (locus %u)", l);
+            max_hap = std::max(max_hap, std::max(sh->ref_len[l], sh->alt_len[l]));
+        }
+        return VTX_OK;
+    };
+    TimeRec* tr = nullptr;
+    int rc = begin_submit(ctx, sh, "vtx_submit_bam", "shard", check, 0, &tr);     // the longest read is known after the record scan
+    if (rc) return rc;
     if (!ctx->stage_stream) {
         CK(cudaStreamCreateWithFlags(&ctx->stage_stream, cudaStreamNonBlocking));
         for (auto& ss : ctx->sslot) { CK(cudaEventCreateWithFlags(&ss.staged, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&ss.free_ev, cudaEventDisableTiming)); }
         ENS(ctx->bam_metrics, sizeof(stage::LocusMetrics));
         CK(cudaMemsetAsync(ctx->bam_metrics.p, 0, sizeof(stage::LocusMetrics), ctx->stage_stream));
-        CK(cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_stage), 256, cudaHostAllocDefault));
+        CK(ctx->h_stage.alloc(256));
     }
     cudaStream_t ss = ctx->stage_stream;
     StageSlot& sl = ctx->sslot[ctx->n_bam_submits & 1];
     ++ctx->n_bam_submits;
     if (sl.used_once) CK(cudaEventSynchronize(sl.free_ev));       // the kernels that read this slot's stream two shards ago are done
     sl.used_once = true;
-    TimeRec* tr = new_trec(ctx);
-    if (!tr) return set_err(ctx, VTX_E_CUDA, "cudaEventCreate failed");
     auto fail_out = [&](int code) { --ctx->trec_used; sl.used_once = false; return code; };
 
     // ---- copies (staging stream) ----
@@ -1238,7 +1260,6 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
         return VTX_OK;
     };
     CK(cudaEventRecord(tr->ev[EV_START], ss));
-    int rc;
     if ((rc = up(sl.comp, sh->comp, sh->comp_len)) || (rc = up(sl.desc, sh->members, size_t(nm) * sizeof(vtx_bgzf_block))) ||
         (rc = up(sl.entry, sh->entry_off, size_t(ne) * 8)) || (rc = up(sl.l_start, sh->locus_start, size_t(nl) * 8)) ||
         (rc = up(sl.l_end, sh->locus_end, size_t(nl) * 8)) || (rc = up(sl.locus_row, sh->locus_row, size_t(nl) * 4)) ||
@@ -1253,13 +1274,7 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
     ENS(sl.status, size_t(nm) * 4 + 16); ENS(sl.scalars, 256);
     uint32_t* d_sc = P<uint32_t>(sl.scalars);       // [0] walk cursor / inflate cursor, [1] err, [2] max_span, [3] max read, [4..] spare
     CK(cudaMemsetAsync(sl.scalars.p, 0, 256, ss));
-    if (nm) {
-        const unsigned ctas = unsigned(std::min<uint64_t>((nm + inflate::kInflateWarps - 1) / inflate::kInflateWarps, uint64_t(ctx->n_sm) * 6));
-        if (int rc_attr = inflate_attr(ctx)) return fail_out(rc_attr);
-        inflate::vtx_k_bgzf_inflate<<<ctas, inflate::kInflateWarps * 32, inflate::inflate_smem_bytes(), ss>>>(P<inflate::BlockDesc>(sl.desc), nm, P<uint8_t>(sl.comp), P<uint8_t>(sl.stream),
-                                                                                 P<int32_t>(sl.status), d_sc, 1);
-        CK(cudaGetLastError());
-    }
+    if (nm && (rc = launch_inflate(ctx, ss, sl.desc.p, nm, sl.comp.p, sl.stream.p, sl.status.p, d_sc, 1))) return fail_out(rc);
     stage::Params sp{};
     sp.s = P<uint8_t>(sl.stream); sp.s_len = stream_len; sp.tid = sh->tid; sp.mapq_min = sh->mapq; sp.primary_only = sh->primary_only;
     sp.no_duplicates = sh->no_duplicates; sp.want_umi = ctx->cfg.use_umi ? 1 : 0; sp.tag0 = uint8_t(sh->bam_tag[0]); sp.tag1 = uint8_t(sh->bam_tag[1]);
@@ -1270,11 +1285,11 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
     std::vector<int32_t> h_status(nm);
     if (n_seg) {
         stage::vtx_k_walk<<<blocks_for(n_seg, stage::kWalkWarps), stage::kWalkWarps * 32, 0, ss>>>(sp, n_seg, P<uint64_t>(sl.entry), 0, P<uint32_t>(sl.seg_count), nullptr, nullptr, d_sc + 1);
-        rc = scan_u32_on(ctx, ss, P<uint32_t>(sl.seg_count), n_seg, P<uint32_t>(sl.seg_first), ctx->stage_sums);
+        rc = scan_u32(ctx, ss, ctx->stage_sums, P<uint32_t>(sl.seg_count), n_seg, P<uint32_t>(sl.seg_first), nullptr);
         if (rc) return fail_out(rc);
     }
     // wait #1 (staging stream only): inflate status, walk errors, number of records
-    uint32_t* hs = reinterpret_cast<uint32_t*>(ctx->h_stage);
+    uint32_t* hs = ctx->h_stage.as<uint32_t>();
     if (n_seg) CK(cudaMemcpyAsync(hs, P<uint32_t>(sl.seg_first) + n_seg, 4, cudaMemcpyDeviceToHost, ss)); else hs[0] = 0;
     CK(cudaMemcpyAsync(hs + 1, d_sc + 1, 4, cudaMemcpyDeviceToHost, ss));
     if (nm) CK(cudaMemcpyAsync(h_status.data(), sl.status.p, size_t(nm) * 4, cudaMemcpyDeviceToHost, ss));
@@ -1304,7 +1319,7 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
         stage::vtx_k_locus_cands<<<blocks_for(nl, 64), 64, 0, ss>>>(sp, nl, P<int64_t>(sl.l_start), P<int64_t>(sl.l_end), n_rec, P<uint64_t>(sl.rec_off),
                                                                    P<int32_t>(sl.rec_tid), P<int32_t>(sl.rec_pos), P<int32_t>(sl.rec_end), P<uint32_t>(sl.rec_fm),
                                                                    d_sc + 2, d_sc + 3, 0, P<uint32_t>(sl.cand_count), nullptr, nullptr, nullptr, d_tmp);
-        rc = scan_u32_on(ctx, ss, P<uint32_t>(sl.cand_count), nl, P<uint32_t>(sl.cand_first), ctx->stage_sums);
+        rc = scan_u32(ctx, ss, ctx->stage_sums, P<uint32_t>(sl.cand_count), nl, P<uint32_t>(sl.cand_first), nullptr);
         if (rc) return fail_out(rc);
         CK(cudaMemcpyAsync(hs, P<uint32_t>(sl.cand_first) + nl, 4, cudaMemcpyDeviceToHost, ss));
     } else hs[0] = 0;
@@ -1389,7 +1404,7 @@ int vtx_wait_copies(vtx_ctx* ctx)
 static int finish_scalars(vtx_ctx* ctx)
 {
     CK(cudaSetDevice(ctx->device));
-    uint64_t* hs = static_cast<uint64_t*>(ctx->h_scalars);
+    uint64_t* hs = ctx->h_scalars.as<uint64_t>();
     CK(cudaMemcpyAsync(hs, ctx->d_res_n.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(hs + 1, ctx->d_metrics.p, 48, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1415,44 +1430,7 @@ int vtx_finish_device(vtx_ctx* ctx, vtx_result* out)
     if (!ctx || !out) return VTX_E_INVALID;
     int rc = finish_scalars(ctx);
     if (rc) return rc;
-    out->n = ctx->last_n;
-    out->row = P<uint32_t>(ctx->r_row); out->col = P<uint32_t>(ctx->r_col); out->ref_cnt = P<uint32_t>(ctx->r_ref);
-    out->alt_cnt = P<uint32_t>(ctx->r_alt); out->unk_cnt = P<uint32_t>(ctx->r_unk);
-    out->val = P<double>(ctx->r_val); out->val2 = P<double>(ctx->r_val2);
-    out->metrics = ctx->last_metrics;
-    return VTX_OK;
-}
-
-static int ensure_host_results(vtx_ctx* ctx, size_t n);
-
-static int fetch_to(vtx_ctx* ctx, const vtx_result* dev, vtx_result* out, void** hbuf, size_t* hcap)
-{
-    const size_t n = dev->n;
-    const size_t esz[7] = { 4, 4, 4, 4, 4, 8, 8 };
-    const bool values_only = (ctx->cfg.flags & VTX_F_VALUES_ONLY) != 0;
-    bool want[7] = { true, true, !values_only, !values_only, !values_only, true, !values_only || ctx->cfg.mode == VTX_MODE_COVERAGE };
-    if (n > *hcap) {
-        const size_t ncap = n + n / 4 + 1024;
-        for (int i = 0; i < 7; ++i) {
-            if (hbuf[i]) { cudaFreeHost(hbuf[i]); hbuf[i] = nullptr; }
-            if (!want[i]) continue;
-            cudaError_t e = cudaHostAlloc(&hbuf[i], ncap * esz[i], cudaHostAllocDefault);
-            if (e != cudaSuccess) { *hcap = 0; return set_err(ctx, VTX_E_NOMEM, "pinned result alloc failed: %s", cudaGetErrorString(e)); }
-        }
-        *hcap = ncap;
-    }
-    const void* src[7] = { dev->row, dev->col, dev->ref_cnt, dev->alt_cnt, dev->unk_cnt, dev->val, dev->val2 };
-    if (n) {
-        for (int i = 0; i < 7; ++i)
-            if (want[i] && src[i]) CK(cudaMemcpyAsync(hbuf[i], src[i], n * esz[i], cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    out->n = n;
-    out->row = static_cast<uint32_t*>(hbuf[0]); out->col = static_cast<uint32_t*>(hbuf[1]);
-    out->ref_cnt = want[2] ? static_cast<uint32_t*>(hbuf[2]) : nullptr; out->alt_cnt = want[3] ? static_cast<uint32_t*>(hbuf[3]) : nullptr;
-    out->unk_cnt = want[4] ? static_cast<uint32_t*>(hbuf[4]) : nullptr;
-    out->val = static_cast<double*>(hbuf[5]); out->val2 = want[6] ? static_cast<double*>(hbuf[6]) : nullptr;
-    out->metrics = dev->metrics;
+    point_result(out, ptrs(ctx->res), 0x7Fu, ctx->last_n, ctx->last_metrics);
     return VTX_OK;
 }
 
@@ -1463,25 +1441,17 @@ int vtx_fetch(vtx_ctx* ctx, const vtx_result* device_result, vtx_result* out)
     CK(cudaSetDevice(ctx->device));
     // gathered results get their own host buffers so that a local and a gathered copy can coexist
     const bool gathered = device_result->row == ctx->g_dev[0].p && ctx->g_dev[0].p != nullptr;
-    return gathered ? fetch_to(ctx, device_result, out, ctx->g_host, &ctx->g_host_cap)
-                    : fetch_to(ctx, device_result, out, ctx->h_res, &ctx->h_res_cap);
-}
-
-// host pinned result arrays with room for `n` triplets
-static int ensure_host_results(vtx_ctx* ctx, size_t n)
-{
-    if (n <= ctx->h_res_cap) return VTX_OK;
-    const size_t esz[7] = { 4, 4, 4, 4, 4, 8, 8 };
-    const size_t ncap = n + n / 4 + 1024;
-    const bool values_only = (ctx->cfg.flags & VTX_F_VALUES_ONLY) != 0;       // then the three count arrays never leave the device
-    const bool want[7] = { true, true, !values_only, !values_only, !values_only, true, !values_only || ctx->cfg.mode == VTX_MODE_COVERAGE };
-    for (int i = 0; i < 7; ++i) {
-        if (ctx->h_res[i]) { cudaFreeHost(ctx->h_res[i]); ctx->h_res[i] = nullptr; }
-        if (!want[i]) continue;
-        cudaError_t e = cudaHostAlloc(&ctx->h_res[i], ncap * esz[i], cudaHostAllocDefault);
-        if (e != cudaSuccess) { ctx->h_res_cap = 0; return set_err(ctx, VTX_E_NOMEM, "pinned result alloc failed: %s", cudaGetErrorString(e)); }
+    HostResults& h = gathered ? ctx->g_host : ctx->h_res;
+    const vtx_result& dev = *device_result;
+    const size_t n = dev.n;
+    int rc = ensure_host(ctx, h, n);
+    if (rc) return rc;
+    if (n) {
+        rc = copy_results(ctx, h, { dev.row, dev.col, dev.ref_cnt, dev.alt_cnt, dev.unk_cnt, dev.val, dev.val2 }, 0, n, ctx->stream);
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));
     }
-    ctx->h_res_cap = ncap;
+    point_result(out, ptrs(h.a), want_mask(ctx), n, dev.metrics);
     return VTX_OK;
 }
 
@@ -1492,22 +1462,18 @@ int vtx_finish(vtx_ctx* ctx, vtx_result* out)
     CK(cudaSetDevice(ctx->device));
     // Stream the triplets out submit by submit: the kernels of later submits are usually still running when the
     // host gets here, so the device->host copy of everything but the last shard hides behind them.
-    const size_t esz[7] = { 4, 4, 4, 4, 4, 8, 8 };
-    DBuf* bufs[7] = { &ctx->r_row, &ctx->r_col, &ctx->r_ref, &ctx->r_alt, &ctx->r_unk, &ctx->r_val, &ctx->r_val2 };
-    const bool values_only = (ctx->cfg.flags & VTX_F_VALUES_ONLY) != 0;
-    const bool want[7] = { true, true, !values_only, !values_only, !values_only, true, !values_only || ctx->cfg.mode == VTX_MODE_COVERAGE };
+    const auto src = ptrs(ctx->res);
     size_t fetched = 0;
-    const bool streamed = !ctx->finished && ctx->h_cum && ctx->fetch_stream && ctx->trec_used > 0 && ctx->trec_used <= kMaxCum;
+    const bool streamed = !ctx->finished && ctx->h_cum.p && ctx->fetch_stream && ctx->trec_used > 0 && ctx->trec_used <= kMaxCum;
     if (streamed) {
-        int rc = ensure_host_results(ctx, ctx->res_ub);
+        int rc = ensure_host(ctx, ctx->h_res, ctx->res_ub);
         if (rc) return rc;
         for (size_t i = 0; i < ctx->trec_used; ++i) {
             CK(cudaEventSynchronize(ctx->trecs[i].ev[EV_POST]));
-            const size_t n_i = size_t(ctx->h_cum[i]);
-            if (n_i > fetched && n_i <= ctx->h_res_cap) {
-                for (int a = 0; a < 7; ++a)
-                    if (want[a]) CK(cudaMemcpyAsync(static_cast<uint8_t*>(ctx->h_res[a]) + fetched * esz[a], static_cast<uint8_t*>(bufs[a]->p) + fetched * esz[a],
-                                                    (n_i - fetched) * esz[a], cudaMemcpyDeviceToHost, ctx->fetch_stream));
+            const size_t n_i = size_t(ctx->h_cum.as<unsigned long long>()[i]);
+            if (n_i > fetched && n_i <= ctx->h_res.cap) {
+                rc = copy_results(ctx, ctx->h_res, src, fetched, n_i, ctx->fetch_stream);
+                if (rc) return rc;
                 fetched = n_i;
             }
         }
@@ -1516,22 +1482,17 @@ int vtx_finish(vtx_ctx* ctx, vtx_result* out)
     int rc = vtx_finish_device(ctx, &dev);
     if (rc) return rc;
     const size_t n = dev.n;
-    rc = ensure_host_results(ctx, n);          // no-op when streamed (res_ub >= n)
+    rc = ensure_host(ctx, ctx->h_res, n);          // no-op when streamed (res_ub >= n)
     if (rc) return rc;
-    if (n > fetched)
-        for (int a = 0; a < 7; ++a)
-            if (want[a]) CK(cudaMemcpyAsync(static_cast<uint8_t*>(ctx->h_res[a]) + fetched * esz[a], static_cast<uint8_t*>(bufs[a]->p) + fetched * esz[a],
-                                            (n - fetched) * esz[a], cudaMemcpyDeviceToHost, ctx->fetch_stream ? ctx->fetch_stream : ctx->stream));
-    CK(cudaStreamSynchronize(ctx->fetch_stream ? ctx->fetch_stream : ctx->stream));
-    out->n = n;
-    out->row = static_cast<uint32_t*>(ctx->h_res[0]); out->col = static_cast<uint32_t*>(ctx->h_res[1]);
-    out->ref_cnt = want[2] ? static_cast<uint32_t*>(ctx->h_res[2]) : nullptr; out->alt_cnt = want[3] ? static_cast<uint32_t*>(ctx->h_res[3]) : nullptr;
-    out->unk_cnt = want[4] ? static_cast<uint32_t*>(ctx->h_res[4]) : nullptr;
-    out->val = static_cast<double*>(ctx->h_res[5]); out->val2 = want[6] ? static_cast<double*>(ctx->h_res[6]) : nullptr;
-    out->metrics = dev.metrics;
+    cudaStream_t st = ctx->fetch_stream ? ctx->fetch_stream : ctx->stream;
+    if (n > fetched) {
+        rc = copy_results(ctx, ctx->h_res, src, fetched, n, st);
+        if (rc) return rc;
+    }
+    CK(cudaStreamSynchronize(st));
+    point_result(out, ptrs(ctx->h_res.a), want_mask(ctx), n, dev.metrics);
     return VTX_OK;
 }
-
 int vtx_last_tile_counts(vtx_ctx* ctx, uint32_t* out, uint32_t n_out)
 {
     if (!ctx || !out) return VTX_E_INVALID;
@@ -1573,9 +1534,8 @@ int vtx_score_pairs(vtx_ctx* ctx, const vtx_batch* hb, uint64_t n_pairs, const u
     Nvtx nvtx_range("vtx_score_pairs");
     if (!ctx) return VTX_E_INVALID;
     if (!hb) return set_err(ctx, VTX_E_INVALID, "batch is NULL");
-    const HostView hv = view_of(hb);
-    HostView hv0 = hv; hv0.n_cand = 0; hv0.cand_read = nullptr;          // the cand_* fields are ignored here
-    int rc = validate_batch(ctx, hv0, false);
+    BatchView hv0 = view_of(hb); hv0.n_cand = 0; hv0.cand_read = nullptr;          // the cand_* fields are ignored here
+    int rc = validate_batch(ctx, hv0);
     if (rc) return rc;
     if (n_pairs >= 0xFFFFFFF0ull) return set_err(ctx, VTX_E_INVALID, "too many pairs");
     if (n_pairs && (!pair_read || !pair_locus || !ref_score || !alt_score)) return set_err(ctx, VTX_E_INVALID, "NULL pair arrays");
@@ -1599,7 +1559,7 @@ int vtx_score_pairs(vtx_ctx* ctx, const vtx_batch* hb, uint64_t n_pairs, const u
     InSlot* sl = nullptr;
     rc = claim_slot(ctx, &sl);
     if (rc) return rc;
-    rc = upload_common(ctx, sl, hb, d);
+    rc = upload_common(ctx, sl, hv0, d);
     if (rc) return rc;
     CK(cudaEventRecord(sl->copy_done, ctx->copy_stream));
     CK(cudaStreamWaitEvent(ctx->stream, sl->copy_done, 0));
@@ -1637,7 +1597,7 @@ uint64_t vtx_pack_umi(const uint8_t* s, uint32_t len)
 
 
 // -------------------------------------------------------------------------------------------------
-// multi-GPU: one allgatherv of the finished triplets over NCCL (NVLink 5 / NVSwitch).  NCCL has no
+// multi-GPU: one allgatherv of the finished triplets over NCCL (NVLink / NVSwitch).  NCCL has no
 // native "v" collective: ncclAllGather of the per-rank counts, then one grouped set of exact-size
 // ncclBroadcast calls (7 arrays x n_ranks roots).  NCCL is dlopen'ed so that single-GPU users (and
 // CPU-only build hosts) never need the library.
@@ -1680,15 +1640,15 @@ bool load_nccl(std::string* why)
     return true;
 }
 #define NK(call) do { int r_ = (call); if (r_ != 0) return set_err(ctx, VTX_E_NCCL, "%s failed: %s", #call, g_nccl.GetErrorString(r_)); } while (0)
-}  // namespace
 
-extern "C" {
-
-void vtx_comm_destroy_internal(vtx_ctx* ctx)
+void comm_destroy(vtx_ctx* ctx)
 {
     if (ctx->comm && g_nccl.ok) g_nccl.CommDestroy(static_cast<nccl_comm>(ctx->comm));
     ctx->comm = nullptr;
 }
+}  // namespace
+
+extern "C" {
 
 int vtx_comm_unique_id(uint8_t id_out[128])
 {
@@ -1725,23 +1685,18 @@ int vtx_gather_start(vtx_ctx* ctx, int32_t root)
     if (root != VTX_GATHER_ALL && (root < 0 || root >= nrk)) return set_err(ctx, VTX_E_INVALID, "gather root %d out of range", root);
     if (nrk != 1 && !ctx->comm) return set_err(ctx, VTX_E_STATE, "vtx_comm_init has not been called");
     CK(cudaSetDevice(ctx->device));
-    const size_t esz[7] = { 4, 4, 4, 4, 4, 8, 8 };
-    DBuf* loc[7] = { &ctx->r_row, &ctx->r_col, &ctx->r_ref, &ctx->r_alt, &ctx->r_unk, &ctx->r_val, &ctx->r_val2 };
-    const bool values_only = (ctx->cfg.flags & VTX_F_VALUES_ONLY) != 0;     // then only row / col / val (/ val2) travel
-    const bool want[7] = { true, true, !values_only, !values_only, !values_only, true, !values_only || ctx->cfg.mode == VTX_MODE_COVERAGE };
+    const uint32_t want = want_mask(ctx);       // only these arrays travel
+    const DBuf* loc = ctx->res;
     vtx_result& out = ctx->g_out;
-    memset(&out, 0, sizeof(out));
-    const void* src[7] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
     if (nrk == 1) {
-        for (int i = 0; i < 7; ++i) if (want[i]) src[i] = loc[i]->p;
-        out.n = ctx->last_n; out.metrics = ctx->last_metrics;
+        point_result(&out, ptrs(ctx->res), want, ctx->last_n, ctx->last_metrics);
     } else {
         if (!ctx->comm_stream) {
             CK(cudaStreamCreateWithFlags(&ctx->comm_stream, cudaStreamNonBlocking));
             CK(cudaEventCreateWithFlags(&ctx->ev_counts, cudaEventDisableTiming));
             CK(cudaEventCreateWithFlags(&ctx->ev_gather, cudaEventDisableTiming));
             CK(cudaEventCreateWithFlags(&ctx->ev_results, cudaEventDisableTiming));
-            CK(cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_counts), size_t(nrk + 1) * 32, cudaHostAllocDefault));
+            CK(ctx->h_counts.alloc(size_t(nrk + 1) * 32));
         }
         cudaStream_t cs = ctx->comm_stream;
         nccl_comm comm = static_cast<nccl_comm>(ctx->comm);
@@ -1751,15 +1706,15 @@ int vtx_gather_start(vtx_ctx* ctx, int32_t root)
         // 1. counts: {n, not_cell_bc, non_umi, scored} of every rank.  One tiny allgather; the host needs the sizes to post
         //    exact-size receives, and waits for this one event only (tens of microseconds, nothing else is blocked).
         ENS(ctx->g_counts, size_t(nrk + 1) * 32);
-        uint64_t* mine = ctx->h_counts + size_t(nrk) * 4;
+        uint64_t* mine = ctx->h_counts.as<uint64_t>() + size_t(nrk) * 4;
         mine[0] = ctx->last_n; mine[1] = ctx->last_metrics.num_not_cell_bc; mine[2] = ctx->last_metrics.num_non_umi; mine[3] = ctx->last_metrics.num_scored;
         uint64_t* dmine = P<uint64_t>(ctx->g_counts) + size_t(nrk) * 4;
         CK(cudaMemcpyAsync(dmine, mine, 32, cudaMemcpyHostToDevice, cs));
         NK(g_nccl.AllGather(dmine, ctx->g_counts.p, 4, kNcclUint64, comm, cs));
-        CK(cudaMemcpyAsync(ctx->h_counts, ctx->g_counts.p, size_t(nrk) * 32, cudaMemcpyDeviceToHost, cs));
+        CK(cudaMemcpyAsync(ctx->h_counts.p, ctx->g_counts.p, size_t(nrk) * 32, cudaMemcpyDeviceToHost, cs));
         CK(cudaEventRecord(ctx->ev_counts, cs));
         CK(cudaEventSynchronize(ctx->ev_counts));
-        const uint64_t* counts = ctx->h_counts;
+        const uint64_t* counts = ctx->h_counts.as<uint64_t>();
         size_t total = 0;
         std::vector<size_t> offs(nrk);
         vtx_metrics met{};
@@ -1767,40 +1722,36 @@ int vtx_gather_start(vtx_ctx* ctx, int32_t root)
             offs[r] = total; total += counts[size_t(r) * 4];
             met.num_not_cell_bc += counts[size_t(r) * 4 + 1]; met.num_non_umi += counts[size_t(r) * 4 + 2]; met.num_scored += counts[size_t(r) * 4 + 3];
         }
-        out.n = total; out.metrics = met;
         const bool receiver = root == VTX_GATHER_ALL || root == ctx->rank;
-        if (receiver) for (int i = 0; i < 7; ++i) if (want[i]) ENS(ctx->g_dev[i], (total ? total : 1) * esz[i]);
+        if (receiver) for (int i = 0; i < kResArrays; ++i) if (want >> i & 1) ENS(ctx->g_dev[i], (total ? total : 1) * kResEsz[i]);
         // 2. the triplets, exact sizes, one NCCL group.  Rooted: ncclSend / ncclRecv, only the writer's GPU receives;
         //    all: one broadcast per (array, rank) = allgatherv.
         NK(g_nccl.GroupStart());
-        for (int i = 0; i < 7; ++i) {
-            if (!want[i]) continue;
+        for (int i = 0; i < kResArrays; ++i) {
+            if (!(want >> i & 1)) continue;
+            const size_t esz = kResEsz[i];
             if (root == VTX_GATHER_ALL) {
                 for (int r = 0; r < nrk; ++r) {
                     const size_t n = counts[size_t(r) * 4];
-                    if (n) NK(g_nccl.Broadcast(loc[i]->p, static_cast<uint8_t*>(ctx->g_dev[i].p) + offs[r] * esz[i], n * esz[i], kNcclUint8, r, comm, cs));
+                    if (n) NK(g_nccl.Broadcast(loc[i].p, static_cast<uint8_t*>(ctx->g_dev[i].p) + offs[r] * esz, n * esz, kNcclUint8, r, comm, cs));
                 }
             } else if (ctx->rank == root) {
                 for (int r = 0; r < nrk; ++r) {
                     const size_t n = counts[size_t(r) * 4];
                     if (!n) continue;
-                    uint8_t* dst = static_cast<uint8_t*>(ctx->g_dev[i].p) + offs[r] * esz[i];
-                    if (r == root) CK(cudaMemcpyAsync(dst, loc[i]->p, n * esz[i], cudaMemcpyDeviceToDevice, cs));
-                    else NK(g_nccl.Recv(dst, n * esz[i], kNcclUint8, r, comm, cs));
+                    uint8_t* dst = static_cast<uint8_t*>(ctx->g_dev[i].p) + offs[r] * esz;
+                    if (r == root) CK(cudaMemcpyAsync(dst, loc[i].p, n * esz, cudaMemcpyDeviceToDevice, cs));
+                    else NK(g_nccl.Recv(dst, n * esz, kNcclUint8, r, comm, cs));
                 }
             } else if (ctx->last_n) {
-                NK(g_nccl.Send(loc[i]->p, size_t(ctx->last_n) * esz[i], kNcclUint8, root, comm, cs));
+                NK(g_nccl.Send(loc[i].p, size_t(ctx->last_n) * esz, kNcclUint8, root, comm, cs));
             }
         }
         NK(g_nccl.GroupEnd());
         CK(cudaEventRecord(ctx->ev_gather, cs));
         ctx->gather_guard = true;
-        if (receiver) for (int i = 0; i < 7; ++i) if (want[i]) src[i] = ctx->g_dev[i].p;
+        point_result(&out, ptrs(ctx->g_dev), receiver ? want : 0u, total, met);
     }
-    out.row = static_cast<const uint32_t*>(src[0]); out.col = static_cast<const uint32_t*>(src[1]);
-    out.ref_cnt = static_cast<const uint32_t*>(src[2]); out.alt_cnt = static_cast<const uint32_t*>(src[3]);
-    out.unk_cnt = static_cast<const uint32_t*>(src[4]);
-    out.val = static_cast<const double*>(src[5]); out.val2 = static_cast<const double*>(src[6]);
     ctx->gather_pending = true;
     return VTX_OK;
 }

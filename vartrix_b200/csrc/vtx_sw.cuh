@@ -174,6 +174,18 @@ __device__ __forceinline__ void call_and_scatter(const SwArgs& a, uint32_t pair,
     atomicAdd(a.counters + size_t(a.pair_slot[pair]) * 4 + k, 1u);
 }
 
+// Dynamic shared memory of one warp of vtx_k_sw_pairs<CLS>: profile, row codes and (multi-pass class) the boundary column.
+// The kernel spells the same sum out inline: calling this helper there changes its instruction schedule.
+template <int CLS>
+__host__ __device__ constexpr size_t sw_warp_bytes(int mcap, int multi)
+{
+    using TC = TileClass<CLS>;
+    constexpr int PPW = 32 / TC::LPP, RS = TC::LPP * TC::CS;
+    const int bnd_stride = (CLS == kMultiClass && multi) ? mcap + 8 : 0;
+    const size_t codes_bytes = (size_t(PPW) * (mcap + 2 * TC::LPP) * 2 + 7) & ~size_t(7);
+    return (size_t(5 * RS) * 4 + codes_bytes + size_t(PPW) * bnd_stride * 8 + 15) & ~size_t(15);
+}
+
 template <int CLS>
 __global__ void __launch_bounds__(TileClass<CLS>::THREADS, TileClass<CLS>::MINB) vtx_k_sw_pairs(const SwArgs a)
 {
@@ -193,7 +205,7 @@ __global__ void __launch_bounds__(TileClass<CLS>::THREADS, TileClass<CLS>::MINB)
     const int code_stride = a.mcap + 2 * M;                      // u16 entries per group
     const int bnd_stride = (MULTI && a.multi) ? a.mcap + 8 : 0;  // uint2 entries per group (multi-pass boundary column)
     const size_t codes_bytes = (size_t(PPW) * code_stride * 2 + 7) & ~size_t(7);
-    const size_t warp_bytes = size_t(5 * RS) * 4 + codes_bytes + size_t(PPW) * bnd_stride * 8;
+    const size_t warp_bytes = size_t(5 * RS) * 4 + codes_bytes + size_t(PPW) * bnd_stride * 8;   // sw_warp_bytes, unrounded
     uint8_t* wbase = smem_raw + warp * ((warp_bytes + 15) & ~size_t(15));
     uint32_t* prof = reinterpret_cast<uint32_t*>(wbase);
     uint16_t* codes = reinterpret_cast<uint16_t*>(wbase + size_t(5 * RS) * 4) + grp * code_stride;
