@@ -97,7 +97,7 @@ def lib():
         L.vtxo_run_batch.restype = ctypes.c_int32
         L.vtxo_run_batch.argtypes = [ctypes.POINTER(CBatch), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32,
                                      ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
-                                     ctypes.POINTER(CResult)]
+                                     ctypes.c_int32, ctypes.POINTER(CResult)]
         L.vtxo_free_result.restype = None
         L.vtxo_free_result.argtypes = [ctypes.POINTER(CResult)]
         _LIB = L
@@ -220,15 +220,19 @@ class Result:
     metrics: dict
 
 
+MIN_SCORE = 25                                               # main.rs:30
+
+
 def run_batch(batch: Batch, barcodes: Barcodes, mode: int, use_umi: bool, n_threads: int = 1,
-              band_model: bool = False) -> Result:
+              band_model: bool = False, min_score: int = MIN_SCORE) -> Result:
+    """min_score: evaluate_scores' MIN_SCORE (a pair is None when both scores are below it), like Engine(min_score=)."""
     L = lib()
     b = batch.normalized()
     cb = b.to_c()
     res = CResult()
     rc = L.vtxo_run_batch(ctypes.byref(cb), barcodes.bytes_.ctypes.data if barcodes.bytes_.size else None,
                           barcodes.off.ctypes.data, len(barcodes), mode, int(use_umi), n_threads,
-                          int(band_model), ctypes.byref(res))
+                          int(band_model), int(min_score), ctypes.byref(res))
     if rc != 0:
         raise RuntimeError(f"vtxo_run_batch failed: {rc}")
     n = int(res.n)

@@ -238,13 +238,18 @@ int32_t vtxo_sw_band_model(const uint8_t* x, int32_t m, const uint8_t* y, int32_
     return ans;
 }
 
-/* main.rs:1019-1030 */
-int32_t vtxo_evaluate_scores(int32_t ref_score, int32_t alt_score)
+/* main.rs:1019-1030; min_score = MIN_SCORE (main.rs:30), a run-time setting of the engine (vtx_config.min_score) */
+static int32_t evaluate_scores(int32_t ref_score, int32_t alt_score, int32_t min_score)
 {
-    if (ref_score < VTXO_MIN_SCORE && alt_score < VTXO_MIN_SCORE) return 0;   /* None */
+    if (ref_score < min_score && alt_score < min_score) return 0;            /* None */
     if (ref_score > alt_score) return 1;                                     /* REF_VALUE */
     if (alt_score > ref_score) return 2;                                     /* ALT_VALUE */
     return -1;                                                               /* UNKNOWN_VALUE */
+}
+
+int32_t vtxo_evaluate_scores(int32_t ref_score, int32_t alt_score)
+{
+    return evaluate_scores(ref_score, alt_score, VTXO_MIN_SCORE);
 }
 
 /* ------------------------------------------------------------------------------------------
@@ -407,7 +412,7 @@ static void evec_push(evec_t* v, entry_t x)
 }
 
 /* parse_scores + convert_to_counts + mode function for one locus (main.rs:1041-1164) */
-static void aggregate_locus(score_t* sc, size_t n, uint32_t row, int32_t mode, int32_t use_umi, evec_t* out)
+static void aggregate_locus(score_t* sc, size_t n, uint32_t row, int32_t mode, int32_t use_umi, int32_t min_score, evec_t* out)
 {
     qsort(sc, n, sizeof(score_t), score_cmp);
     size_t i = 0;
@@ -416,7 +421,7 @@ static void aggregate_locus(score_t* sc, size_t n, uint32_t row, int32_t mode, i
         uint32_t r = 0, a = 0, u = 0;
         if (!use_umi) {
             for (size_t k = i; k < j; ++k) {                              /* main.rs:1090-1098 */
-                int32_t c = vtxo_evaluate_scores(sc[k].rs, sc[k].as);
+                int32_t c = evaluate_scores(sc[k].rs, sc[k].as, min_score);
                 if (c == 1) ++r; else if (c == 2) ++a; else if (c == -1) ++u;
             }
         } else {
@@ -427,7 +432,7 @@ static void aggregate_locus(score_t* sc, size_t n, uint32_t row, int32_t mode, i
                 if (seen) continue;
                 uint32_t ur = 0, ua = 0, uu = 0;
                 for (size_t q = k; q < j; ++q) if (sc[q].umi == sc[k].umi) {
-                    int32_t c = vtxo_evaluate_scores(sc[q].rs, sc[q].as);
+                    int32_t c = evaluate_scores(sc[q].rs, sc[q].as, min_score);
                     if (c == 1) ++ur; else if (c == 2) ++ua; else if (c == -1) ++uu;
                 }
                 uint32_t t = ur + ua + uu;
@@ -455,7 +460,7 @@ static void aggregate_locus(score_t* sc, size_t n, uint32_t row, int32_t mode, i
 }
 
 typedef struct {
-    const vtxo_batch* b; const bcmap_t* bc; uint32_t lo, hi; int32_t mode, use_umi, band;
+    const vtxo_batch* b; const bcmap_t* bc; uint32_t lo, hi; int32_t mode, use_umi, band, min_score;
     evec_t out; vtxo_metrics met;
 } rb_job;
 
@@ -490,7 +495,7 @@ static void rb_chunk(rb_job* J)
             }
             ++n; J->met.num_scored++;
         }
-        aggregate_locus(sc, n, b->locus_row[l], J->mode, J->use_umi, &J->out);
+        aggregate_locus(sc, n, b->locus_row[l], J->mode, J->use_umi, J->min_score, &J->out);
     }
     free(sc); free(seq);
 }
@@ -512,7 +517,7 @@ static void* rb_worker(void* arg)
 int32_t vtxo_run_batch(const vtxo_batch* b,
                        const uint8_t* bc_bytes, const uint32_t* bc_off, uint32_t n_barcodes,
                        int32_t mode, int32_t use_umi, int32_t n_threads, int32_t use_band_model,
-                       vtxo_result* out)
+                       int32_t min_score, vtxo_result* out)
 {
     memset(out, 0, sizeof(*out));
     bcmap_t bc; bcmap_build(&bc, bc_bytes, bc_off, n_barcodes);
@@ -525,7 +530,7 @@ int32_t vtxo_run_batch(const vtxo_batch* b,
     pthread_t* th = (pthread_t*)malloc(sizeof(pthread_t) * (n_chunks ? n_chunks : 1));
     for (uint32_t c = 0; c < n_chunks; ++c) {
         jobs[c].b = b; jobs[c].bc = &bc; jobs[c].lo = c * chunk; jobs[c].hi = imin((int32_t)(c * chunk + chunk), (int32_t)n);
-        jobs[c].mode = mode; jobs[c].use_umi = use_umi; jobs[c].band = use_band_model;
+        jobs[c].mode = mode; jobs[c].use_umi = use_umi; jobs[c].band = use_band_model; jobs[c].min_score = min_score;
     }
     uint32_t next = 0; rb_pool pool = { jobs, n_chunks, &next };
     uint32_t nt = (uint32_t)n_threads < n_chunks ? (uint32_t)n_threads : n_chunks;

@@ -80,7 +80,7 @@ int32_t vtxo_sw_fold(const uint8_t* x, int32_t m, const uint8_t* y, int32_t n, i
  * DIAGNOSTIC ONLY -- used to count pairs whose banded score could differ from the full one. */
 int32_t vtxo_sw_band_model(const uint8_t* x, int32_t m, const uint8_t* y, int32_t n, int32_t k, int32_t w);
 
-/* main.rs:1019-1030 : 0 = None, 1 = REF, 2 = ALT, -1 = UNKNOWN */
+/* main.rs:1019-1030 with MIN_SCORE = VTXO_MIN_SCORE : 0 = None, 1 = REF, 2 = ALT, -1 = UNKNOWN */
 int32_t vtxo_evaluate_scores(int32_t ref_score, int32_t alt_score);
 
 /* rust-htslib 0.36 CigarStringView::read_pos(p, false, true) folded into main.rs:790-806.
@@ -98,6 +98,8 @@ int32_t vtxo_score_pairs(const vtxo_batch* b, uint64_t n_pairs, const uint32_t* 
 /* Whole path for a staged batch: CB lookup (main.rs:737-750), UMI gate (879-888), 2x SW (898-901),
  * stable sort by cell (932), parse_scores (1041-1109), mode function (1111-1164), row-major merge
  * (320-348).  Loci are split into static contiguous chunks of max(n/threads,1) like main.rs:250-254.
+ * min_score is MIN_SCORE of evaluate_scores (main.rs:30, 1019-1030): VTXO_MIN_SCORE in the reference, a run-time
+ * setting of the engine (vtx_config.min_score) that this argument mirrors.
  * Output arrays are malloc'ed by the library; free with vtxo_free_result. */
 typedef struct vtxo_result {
     uint64_t  n;          /* entries */
@@ -114,7 +116,7 @@ typedef struct vtxo_result {
 int32_t vtxo_run_batch(const vtxo_batch* b,
                        const uint8_t* bc_bytes, const uint32_t* bc_off, uint32_t n_barcodes,
                        int32_t mode, int32_t use_umi, int32_t n_threads, int32_t use_band_model,
-                       vtxo_result* out);
+                       int32_t min_score, vtxo_result* out);
 void vtxo_free_result(vtxo_result* r);
 
 #ifdef __cplusplus

@@ -11,27 +11,32 @@ from conftest import assert_same_triplets, to_oracle_batch
 pytestmark = pytest.mark.gpu
 
 
-def _run(oracle, cfg, n_submits):
+def _run(oracle, cfg, n_submits, engine_flags=({},)):
+    """the oracle once; the engine once per entry of engine_flags (Engine keyword arguments)"""
     import vartrix_b200 as vb
     sb, bcs, info = vb.synth.make_shard(**cfg)
     umi = bool(cfg.get("umi"))
-    with vb.Engine(cfg["scoring_method"], umi=umi) as eng:
-        eng.set_barcodes(bcs)
-        for lo, hi in vb.shard_bounds(sb.cand_start, n_submits):
-            eng.submit(sb.shard(lo, hi))
-        got = eng.finish()
     exp = oracle.run_batch(to_oracle_batch(oracle, sb), oracle.Barcodes(bcs.keys), oracle.MODES[cfg["scoring_method"]], umi,
                            n_threads=len(os.sched_getaffinity(0)))
-    assert_same_triplets(got, exp)
-    assert got.metrics == exp.metrics
-    assert got.metrics["num_scored"] == info["n_pairs"]
+    for kw in engine_flags:
+        with vb.Engine(cfg["scoring_method"], umi=umi, **kw) as eng:
+            eng.set_barcodes(bcs)
+            for lo, hi in vb.shard_bounds(sb.cand_start, n_submits):
+                eng.submit(sb.shard(lo, hi))
+            got = eng.finish()
+        assert_same_triplets(got, exp)
+        assert got.metrics == exp.metrics, kw
+        assert got.metrics["num_scored"] == info["n_pairs"], kw
     return got, info
 
 
 @pytest.mark.parametrize("name,n_submits", [("config2", 3), ("config4", 4), ("config3", 5)])
 def test_full_config_bit_exact(oracle, name, n_submits):
     import vartrix_b200 as vb
-    got, info = _run(oracle, dict(vb.synth.CONFIGS[name]), n_submits)
+    # config 2 also through the two-phase kernels alone (no_fold) and the single-phase classes alone (no_split): the
+    # whole pipeline (slots, counts) at full size through those kernels (chunked tiles: tests/test_gpu_sw_scale.py)
+    flags = ({}, dict(no_fold=True), dict(no_split=True)) if name == "config2" else ({},)
+    got, info = _run(oracle, dict(vb.synth.CONFIGS[name]), n_submits, flags)
     assert len(got.row) > 0.8 * info["n_pairs"]          # ~1 read per cell at these barcode counts
 
 
