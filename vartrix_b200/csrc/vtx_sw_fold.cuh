@@ -15,9 +15,10 @@
 //
 //   main pass   kFoldP = 96 columns, 12 per lane, rows skewed by one step per lane exactly like the other
 //               kernels -- but the two int16 halves are (forward DP over hap[0, 96), reversed DP over
-//               hap[n - 96, n) reversed) of the SAME read.  Per step a lane fetches the forward and the reverse
-//               profile row (LDS.128) and merges them with an IMAD.  The last column (H + gap, E) of every
-//               row goes to shared memory.
+//               hap[n - 96, n) reversed) of the SAME read.  Forward row i and reversed row i are read rows i and
+//               m - 1 - i, so the per-locus profile is pre-merged over the pair of their codes (25 rows): per
+//               step a lane loads one pair code and its 12 substitution words (3 LDS.128), nothing to merge.
+//               The last column (H + gap, E) of every row goes to shared memory.
 //   middle      the n - 192 allele columns (9 for an SNV with --padding 100, up to 40): halves are (ref, alt)
 //               again.  Transposed wavefront: lane g owns the 19 read rows [19 g, 19 g + 19), whose (H + gap, E)
 //               start from the parked forward boundary, and walks over the columns one step per column,
@@ -42,21 +43,22 @@ constexpr int kFoldMaxMid = 40;        // allele columns: n <= 2 * 96 + 40 = 232
 // boundary rows kept per read; 156 (not 152) so that the four reads of a tile start 8, 16 and 24 banks apart
 // (152 rows x 8 bytes put reads 0/2 and 1/3 on the same banks: a 2-way conflict on every boundary store and load)
 constexpr int kFoldRows = kFoldMaxRead + 4;
-constexpr int kFoldCodeStride = kFoldMaxRead + 16;   // row codes per read and direction (8 sentinels either side)
-// 288 threads x 2 CTAs = 18 warps/SM at 96 registers (a few spills in the tile prologue only); the kernel is bound by issue
-// slots and the ALU pipe, not by latency, so more resident warps buy little and fewer registers would cost spills.
+constexpr int kFoldCodeStride = kFoldMaxRead + 16;   // row codes per read and kind (8 sentinels either side)
+constexpr int kFoldPairRows = 25;                    // merged profile rows: 5 x forward code + reverse code
 #ifndef VTX_FOLD_UNROLL
-#define VTX_FOLD_UNROLL 2
+#define VTX_FOLD_UNROLL 4
 #endif
-// 1: the reverse profile is stored in the HIGH half, so the (forward | reverse) substitution word is a plain add of the two
-// profile words (eligible for IMAD.IADD / VIADD) instead of a full IMAD b * 65536 + a (half-rate FMA-heavy pipe)
-#ifndef VTX_FOLD_PRESHIFT
-#define VTX_FOLD_PRESHIFT 0
-#endif
+// 17 248 B of shared memory per warp: one CTA of 416 threads = 13 warps/SM (124 registers, no spills at unroll 4).
+// Measured on H100 (profiles/h100_fold_profile_ceiling.txt): 2 x 192 threads = 12 warps/SM is 2.6 % slower, and unroll 2
+// (the choice at 18 warps) 1.3 % slower; unroll 1 costs 10 %.
 #ifndef VTX_FOLD_THREADS
-#define VTX_FOLD_THREADS 288
+#define VTX_FOLD_THREADS 416
+#endif
+#ifndef VTX_FOLD_BLOCKS
+#define VTX_FOLD_BLOCKS 1
 #endif
 constexpr int kFoldThreads = VTX_FOLD_THREADS;
+constexpr int kFoldBlocks = VTX_FOLD_BLOCKS;          // resident CTAs per SM that __launch_bounds__ plans registers for
 constexpr int kFoldUnroll = VTX_FOLD_UNROLL;         // row-loop unrolling of the main pass
 #ifndef VTX_FOLD_MID_UNROLL
 #define VTX_FOLD_MID_UNROLL 1
@@ -65,10 +67,10 @@ constexpr int kFoldMidUnroll = VTX_FOLD_MID_UNROLL;  // column-loop unrolling of
 
 __host__ __device__ constexpr size_t fold_warp_bytes()
 {
-    size_t b = size_t(2 * 5 * kFoldP) * 4;                       // forward + reverse profile
+    size_t b = size_t(kFoldPairRows * kFoldP) * 4;              // merged profile [pair code][column]
     b += size_t(kFoldMaxMid) * 8 * 4;                            // allele-column table [column][read code]
     b += size_t(kFoldPPW) * kFoldRows * 8 + 32;                  // boundary column (forward | reverse), per read and row
-    b += size_t(2 * kFoldPPW) * kFoldCodeStride;                 // row codes, forward and reversed
+    b += size_t(2 * kFoldPPW) * kFoldCodeStride;                 // row codes: forward, and pair (row i, row m - 1 - i)
     return (b + 15) & ~size_t(15);
 }
 
@@ -78,7 +80,7 @@ constexpr int kJuncH = -2 * kGoe - kBias, kJuncE = -kGapOpen - kBias;
 constexpr uint32_t kJuncH2 = (uint32_t(uint16_t(int16_t(kJuncH - 1))) << 16) | uint32_t(uint16_t(int16_t(kJuncH)));
 constexpr uint32_t kJuncE2 = (uint32_t(uint16_t(int16_t(kJuncE - 1))) << 16) | uint32_t(uint16_t(int16_t(kJuncE)));
 
-__global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
+__global__ void __launch_bounds__(kFoldThreads, kFoldBlocks) vtx_k_sw_fold(const SwArgs a)
 {
     constexpr int C1 = kFoldC1, P = kFoldP, R = kFoldR, M = 8;
     constexpr int RS1 = P;                                       // 96 words: rows stay on their banks
@@ -87,16 +89,14 @@ __global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int u = lane >> 3, g = lane & 7;                       // unit = read of the tile, lane within the unit
     uint8_t* wbase = smem_raw + warp * fold_warp_bytes();
-    uint32_t* profF = reinterpret_cast<uint32_t*>(wbase);
-    uint32_t* profR = profF + 5 * RS1;
-    uint32_t* midtab = profR + 5 * RS1;
+    uint32_t* prof = reinterpret_cast<uint32_t*>(wbase);
+    uint32_t* midtab = prof + kFoldPairRows * RS1;
     uint2* bnd = reinterpret_cast<uint2*>(midtab + kFoldMaxMid * 8);
     uint8_t* codes = reinterpret_cast<uint8_t*>(bnd + kFoldPPW * kFoldRows + 4);
 
     const uint32_t n_tiles = __ldg(a.tile_start + a.n_loci);
     uint32_t cached_locus = 0xFFFFFFFFu;
     const uint32_t tile_chunk = max(1u, min(uint32_t(kTileChunk), n_tiles / (gridDim.x * (blockDim.x >> 5) * 16u)));
-    const uint32_t k64k = a.k64k;                                // 65536, opaque to ptxas so the merge stays an IMAD
     const uint32_t one = a.one;
     int mid_ref = 0, mid_alt = 0;                                // allele columns of the cached locus
 
@@ -121,14 +121,25 @@ __global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
                 const int n_ref = int(__ldg(a.ref_len + locus)), n_alt = int(__ldg(a.alt_len + locus));
                 mid_ref = n_ref - 2 * P;
                 mid_alt = n_alt - 2 * P;
-                for (int j = lane; j < P; j += 32) {             // both flanks are common to ref and alt (vtx_k_locus_prep)
-                    const uint32_t fb = hap_code(__ldg(rh + j));
-                    const uint32_t sb = hap_code(__ldg(rh + (n_ref - 1 - j)));
+                // row 5 a + b, column c: {s(a, hap[c]), s(b, hap[n - 1 - c])}; both flanks are common to ref and alt
+                // (vtx_k_locus_prep).  Lane j < 24 fills columns [4 j, 4 j + 4) of every row with one STS.128 each.
+                if (lane < P / 4) {
+                    uint32_t fb[4], sb[4];
 #pragma unroll
-                    for (uint32_t r = 0; r < 5; ++r) {
-                        profF[r * RS1 + j] = uint32_t(r == fb ? kProfMatch : kProfMis);      // low half only: merged per step
-                        profR[r * RS1 + j] = uint32_t(r == sb ? kProfMatch : kProfMis) << (VTX_FOLD_PRESHIFT ? 16 : 0);
+                    for (int k = 0; k < 4; ++k) {
+                        fb[k] = hap_code(__ldg(rh + 4 * lane + k));
+                        sb[k] = hap_code(__ldg(rh + (n_ref - 1 - 4 * lane - k)));
                     }
+#pragma unroll
+                    for (uint32_t ra = 0; ra < 5; ++ra)
+#pragma unroll
+                        for (uint32_t rb = 0; rb < 5; ++rb) {
+                            uint32_t w[4];
+#pragma unroll
+                            for (int k = 0; k < 4; ++k)
+                                w[k] = pack2(ra == fb[k] ? kProfMatch : kProfMis, rb == sb[k] ? kProfMatch : kProfMis);
+                            reinterpret_cast<uint4*>(prof + (5 * ra + rb) * RS1)[lane] = make_uint4(w[0], w[1], w[2], w[3]);
+                        }
                 }
                 const int lmax = max(mid_ref, mid_alt);
                 for (int idx = lane; idx < lmax * 8; idx += 32) {
@@ -139,10 +150,12 @@ __global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
                     midtab[idx] = pack2(r == rb ? kProfMatch : kProfMis, r == ab ? kProfMatch : kProfMis);
                 }
             }
-            // ---- row codes, forward and reversed: the 8 lanes of a unit fill their read ----
+            // ---- row codes: the 8 lanes of a unit fill their read's forward codes, then the pair codes from them ----
             const uint32_t pair = p0 + u;
             const bool active = pair < p_end;
             int m = 0;
+            uint8_t* cf = codes + (2 * u) * kFoldCodeStride;                 // forward code of row e - M (the middle's rows)
+            uint8_t* cp = cf + kFoldCodeStride;                               // 5 x code(row e - M) + code(row m - 1 - (e - M))
             {
                 const uint8_t* nib = nullptr;
                 if (active) {
@@ -150,17 +163,16 @@ __global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
                     m = int(__ldg(a.read_len + rd));
                     nib = a.read_nib + __ldg(a.read_off + rd);
                 }
-                uint8_t* cf = codes + (2 * u) * kFoldCodeStride;
-                uint8_t* cr = cf + kFoldCodeStride;
                 for (int e = g; e < kFoldCodeStride; e += 8)
-                    if (e < M || e >= M + m) { cf[e] = 4; cr[e] = 4; }
+                    if (e < M || e >= M + m) cf[e] = 4;
                 for (int b = g; 2 * b < m; b += 8) {
                     const uint32_t by = __ldg(nib + b);
-                    const uint8_t c0 = uint8_t(nib_code(by >> 4)), c1 = uint8_t(nib_code(by & 0xF));
-                    cf[M + 2 * b] = c0;
-                    cr[M + m - 1 - 2 * b] = c0;
-                    if (2 * b + 1 < m) { cf[M + 2 * b + 1] = c1; cr[M + m - 2 - 2 * b] = c1; }
+                    cf[M + 2 * b] = uint8_t(nib_code(by >> 4));
+                    if (2 * b + 1 < m) cf[M + 2 * b + 1] = uint8_t(nib_code(by & 0xF));
                 }
+                __syncwarp();
+                for (int e = g; e < kFoldCodeStride; e += 8)                 // sentinel rows: (4, 4), all mismatch
+                    cp[e] = (e < M || e >= M + m) ? uint8_t(5 * 4 + 4) : uint8_t(5 * cf[e] + cf[2 * M + m - 1 - e]);
             }
             int mmax = m;
 #pragma unroll
@@ -180,30 +192,22 @@ __global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
                 for (int c = 0; c < C1; ++c) { hg[c] = kGOE2; f[c] = kNEG2; }
                 uint32_t hg_last = kGOE2, e_last = kNEG2, diag_save = kGOE2;
                 best = kBIAS2;
-                const uint8_t* cA = codes + (2 * u) * kFoldCodeStride + M - g;
-                const uint8_t* cB = cA + kFoldCodeStride;
-                const uint32_t* lane_f = profF + g * C1;
-                const uint32_t* lane_r = profR + g * C1;
+                const uint8_t* cA = cp + M - g;
+                const uint32_t* lane_p = prof + g * C1;
                 const int steps = mmax + 7;
 #pragma unroll kFoldUnroll
                 for (int t = 0; t < steps; ++t) {
                     uint32_t hl = __shfl_up_sync(0xffffffffu, hg_last, 1, 8);
                     uint32_t el = __shfl_up_sync(0xffffffffu, e_last, 1, 8);
                     if (g == 0) { hl = kGOE2; el = kNEG2; }
-                    const uint4* pa = reinterpret_cast<const uint4*>(lane_f + uint32_t(cA[t]) * RS1);
-                    const uint4* pb = reinterpret_cast<const uint4*>(lane_r + uint32_t(cB[t]) * RS1);
+                    const uint4* pa = reinterpret_cast<const uint4*>(lane_p + uint32_t(cA[t]) * RS1);
                     uint32_t diag = diag_save;
                     diag_save = hl;
                     uint32_t e = el, eg = hl, hleft = hl;
 #pragma unroll
                     for (int q = 0; q < C1 / 4; ++q) {
-                        const uint4 a4 = pa[q], b4 = pb[q];
-                        // {s_fwd, s_rev} = s_fwd + (s_rev << 16) as an IMAD (FMA pipe), like vtx_k_sw_split's phase 1
-#if VTX_FOLD_PRESHIFT
-                        const uint32_t sv[4] = { b4.x + a4.x, b4.y + a4.y, b4.z + a4.z, b4.w + a4.w };
-#else
-                        const uint32_t sv[4] = { b4.x * k64k + a4.x, b4.y * k64k + a4.y, b4.z * k64k + a4.z, b4.w * k64k + a4.w };
-#endif
+                        const uint4 a4 = pa[q];                                      // {s_fwd, s_rev}
+                        const uint32_t sv[4] = { a4.x, a4.y, a4.z, a4.w };
                         uint32_t hh[4];
 #pragma unroll
                         for (int k = 0; k < 4; ++k) {
@@ -236,7 +240,7 @@ __global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
                 const int lmax = max(mid_ref, mid_alt), lmin = min(mid_ref, mid_alt);
                 const uint32_t short_mask = mid_ref < mid_alt ? 0x0000FFFFu : 0xFFFF0000u;   // half whose allele ends first
                 uint32_t hg[R], e[R], rc[R];
-                const uint8_t* cf = codes + (2 * u) * kFoldCodeStride + M + R * g;
+                const uint8_t* cfm = cf + M + R * g;
 #pragma unroll
                 for (int c = 0; c < R; ++c) {
                     const int row = R * g + c;
@@ -244,7 +248,7 @@ __global__ void __launch_bounds__(kFoldThreads, 2) vtx_k_sw_fold(const SwArgs a)
                     if (row < mmax) b = row_bnd[row];
                     hg[c] = __byte_perm(b.x, 0, 0x1010);                             // forward half, for ref and alt
                     e[c] = __byte_perm(b.y, 0, 0x1010);
-                    rc[c] = uint32_t(cf[c]) * 4u;
+                    rc[c] = uint32_t(cfm[c]) * 4u;
                 }
                 // junction of the halves in `mask`: forward row r meets reversed row m - 2 - r
                 auto junction = [&](uint32_t mask) {
