@@ -1,5 +1,5 @@
 """Kernel-tuning aid: time the device-resident hot path with alternative builds of the library (VTX_LIB).
-    python tools/sw_variant_bench.py --loci 30000 build/variants/lib_*.so
+    python tools/sw_variant_bench.py --loci 30000 [--depth 50] build/variants/lib_*.so
 One shard is generated once; every build runs in its own process on the same data."""
 import argparse
 import json
@@ -49,6 +49,7 @@ def main():
     ap.add_argument("libs", nargs="*")
     ap.add_argument("--loci", type=int, default=30000)
     ap.add_argument("--kind", default="snv")
+    ap.add_argument("--depth", type=int, default=50, help="reads per locus (4: one fold tile per locus)")
     ap.add_argument("--umi", action="store_true")
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--child", default="")
@@ -56,7 +57,7 @@ def main():
     if a.child:
         return child(a.child, a.steps)
     import vartrix_b200 as vb
-    sb, bcs, info = vb.synth.make_shard(a.loci, 5000, seed=1, kind=a.kind, umi=a.umi)
+    sb, bcs, info = vb.synth.make_shard(a.loci, 5000, depth=a.depth, seed=1, kind=a.kind, umi=a.umi)
     npz = "/tmp/vtx_variant_shard.npz"
     np.savez(npz, n_rows=sb.n_rows, keys=np.array([np.frombuffer(k, np.uint8) for k in bcs.keys]), mode="coverage", umi=a.umi,
              **{f: getattr(sb, f) for f in vb.StagedBatch.FIELDS})

@@ -330,10 +330,9 @@ SwAllow sw_allow(const vtx_ctx* ctx, uint32_t max_read, uint32_t max_hap)
 }
 // A persistent grid of a Smith-Waterman kernel: as many blocks as fit on every SM at once, each warp taking tiles from
 // a.tile_counter until none are left.  `name` / `cls` (-1: none) name the kernel in the error message.
-int launch_sw(vtx_ctx* ctx, void (*kern)(SwArgs), int threads, size_t warp_bytes, const SwArgs& a, uint64_t* launches,
+int launch_sw(vtx_ctx* ctx, void (*kern)(SwArgs), int threads, size_t smem, const SwArgs& a, uint64_t* launches,
               const char* name, int cls)
 {
-    const size_t smem = warp_bytes * (threads / 32);
     CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
     int per_sm = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
@@ -349,13 +348,19 @@ int launch_sw(vtx_ctx* ctx, void (*kern)(SwArgs), int threads, size_t warp_bytes
 
 template <int CLS> int launch_sw_class(vtx_ctx* ctx, const SwArgs& a, uint64_t* launches)
 {
-    return launch_sw(ctx, vtx_k_sw_pairs<CLS>, TileClass<CLS>::THREADS, sw_warp_bytes<CLS>(a.mcap, a.multi), a, launches,
+    return launch_sw(ctx, vtx_k_sw_pairs<CLS>, TileClass<CLS>::THREADS,
+                     sw_warp_bytes<CLS>(a.mcap, a.multi) * (TileClass<CLS>::THREADS / 32), a, launches,
                      "SW kernel class", CLS);
 }
 template <int SCLS> int launch_sw_split(vtx_ctx* ctx, const SwArgs& a, uint64_t* launches)
 {
-    return launch_sw(ctx, vtx_k_sw_split<SCLS>, SplitClass<SCLS>::THREADS, split_warp_bytes<SCLS>(a.mcap), a, launches,
+    return launch_sw(ctx, vtx_k_sw_split<SCLS>, SplitClass<SCLS>::THREADS,
+                     split_warp_bytes<SCLS>(a.mcap) * (SplitClass<SCLS>::THREADS / 32), a, launches,
                      "split SW kernel", SCLS);
+}
+template <int W, int S, bool SHARED> int launch_sw_fold(vtx_ctx* ctx, const SwArgs& a, uint64_t* launches)
+{
+    return launch_sw(ctx, vtx_k_sw_fold<W, S, SHARED>, W * 32, fold_cta_bytes<W, S>(), a, launches, "folded SW kernel", -1);
 }
 
 // classes + tiles + SW kernels, shared by submit and score_pairs.  pair_start must be ready.
@@ -450,7 +455,12 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
     if (allow.fold && (b.class_mask >> kFoldClass & 1u)) {
         a.tile_start = P<uint32_t>(ctx->tstart) + size_t(kFoldClass) * (nl + 1);
         a.tile_counter = P<uint32_t>(ctx->tile_counters) + kFoldClass;
-        int rc = launch_sw(ctx, vtx_k_sw_fold, kFoldThreads, fold_warp_bytes(), a, launches, "folded SW kernel", -1);
+        // the depth is taken over all candidates and loci of the shard, which the host knows for host and device
+        // batches alike, not over fold tiles: shallow fold loci in a shard of deep loci of other kernels run the deep
+        // shape, which is slower on 1-tile loci but still exact
+        const bool deep = uint64_t(n_pairs_ub) >= uint64_t(kFoldDeepDepth) * nl;
+        int rc = deep ? launch_sw_fold<kFoldDeepWarps, kFoldDeepSlots, true>(ctx, a, launches)
+                      : launch_sw_fold<kFoldShallowWarps, kFoldShallowWarps, false>(ctx, a, launches);
         if (rc) return rc;
     }
     if (b.class_mask >> kSlowClass & 1u) {   // generic class (rare)
