@@ -86,6 +86,10 @@ typedef struct vtx_config {
 #define VTX_F_VALUES_ONLY 4u    /* vtx_finish / vtx_fetch copy only row, col, val (and val2 in coverage mode) to the host;
                                    ref_cnt / alt_cnt / unk_cnt come back NULL (halves the device->host traffic) */
 #define VTX_F_NO_FOLD     8u    /* do not use the folded (shared prefix AND suffix) Smith-Waterman kernel */
+#define VTX_F_NAME_KEYS  16u    /* vtx_submit_bam keys reads by QNAME, not UB: the records of one template inside one (locus, cell)
+                                   are collapsed like the reads of one UMI (--collapse-mates); a QNAME of "*" is a key of its own.
+                                   Needs use_umi (vtx_create returns VTX_E_INVALID otherwise).  Host batches are unaffected: their
+                                   caller supplies the name keys in read_umi_key. */
 
 /*
  * One staged shard of loci.  SoA; for vtx_submit the pointers are HOST pointers (ideally pinned, see
@@ -102,7 +106,9 @@ typedef struct vtx_config {
  *               to a multiple of 16 bytes.
  * cb / umi    : per read.  CB bytes are compared by exact byte equality with the barcode list.
  *               read_umi_key is any injective encoding of the UB string into [0, VTX_UMI_KEY_MAX]
- *               (equal key <=> equal bytes inside one ctx run); see vtx_pack_umi.
+ *               (equal key <=> equal bytes inside one ctx run); see vtx_pack_umi.  To count each template once
+ *               per cell (--collapse-mates), key the reads by QNAME instead: keys only meet inside one locus, so
+ *               any code that is injective within the shard will do, with a fresh key for every QNAME "*".
  * candidates  : (read, locus) pairs that survived the host-side filters, locus-major, BAM file order
  *               inside a locus (order only matters for reproducing metrics, not matrices).
  */
@@ -271,7 +277,9 @@ int         vtx_bgzf_inflate(vtx_ctx* ctx, const vtx_bgzf_block* blocks, uint32_
  * csrc/host/stager.hpp does on staging threads and the reference does through rust-htslib: every record of contig `tid`
  * with pos < end and bam_endpos > start per locus, in file order (main.rs:822-829); mapq / primary / duplicate /
  * useful_alignment filters in that order (main.rs:833-865); CB (`bam_tag`) and UB as the first Z-typed aux field of that
- * name (main.rs:737-757); then the same pipeline as vtx_submit.  Loci must be ascending on one contig of a
+ * name (main.rs:737-757) -- with VTX_F_NAME_KEYS the QNAME instead of UB, interned on the device (a hash table of record
+ * indices: key = the index of the first record with that name; "*" keeps its own index); then the same pipeline as
+ * vtx_submit.  Loci must be ascending on one contig of a
  * coordinate-sorted BAM.  Asynchronous like vtx_submit (two short waits on the staging stream for sizes).
  *   members / comp : as for vtx_bgzf_inflate, in file order, out_off = running sum of out_len (one contiguous stream)
  *   entry_off      : ascending offsets into that stream; [0] = first record to look at, [n_entry - 1] = end of the

@@ -22,6 +22,7 @@ F_KEEP_SCORES = 1
 F_NO_SPLIT = 2
 F_VALUES_ONLY = 4
 F_NO_FOLD = 8
+F_NAME_KEYS = 16        # vtx_submit_bam keys reads by QNAME instead of UB (--collapse-mates); needs use_umi
 
 # every symbol include/vartrix_b200.h declares (tests check the library exports all of them)
 SYMBOLS = [

@@ -49,7 +49,7 @@ struct Opts {
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
     std::vector<int> devices;          // --devices: the loci are sharded over these GPUs (contiguous ranges, main.rs:250-254)
-    bool primary = false, no_dups = false, umi = false, ref_matrix_given = false, gpu_inflate = false, gpu_stage = false, cut_at_contigs = false;
+    bool primary = false, no_dups = false, umi = false, collapse_mates = false, ref_matrix_given = false, gpu_inflate = false, gpu_stage = false, cut_at_contigs = false;
 };
 
 void usage()
@@ -72,6 +72,8 @@ void usage()
          "      --primary-alignments    Use primary alignments only\n"
          "      --no-duplicates         Do not consider duplicate alignments\n"
          "      --umi                   Consider UMI information\n"
+         "      --collapse-mates        Count each paired-end fragment once per cell: the records of one QNAME at a locus are\n"
+         "                              collapsed like the reads of one UMI (not with --umi, which already collapses mates)\n"
          "      --bam-tag TAG           BAM tag marking cells [CB]\n"
          "      --valid-chars CHARS     Valid characters in an alternative haplotype [ATGCatgc]\n"
          "      --device INT            CUDA device ordinal [0]\n"
@@ -132,6 +134,7 @@ bool parse(int argc, char** argv, Opts* o)
         else if (a == "--primary-alignments") o->primary = true;
         else if (a == "--no-duplicates") o->no_dups = true;
         else if (a == "--umi") o->umi = true;
+        else if (a == "--collapse-mates") o->collapse_mates = true;
         else if (a == "--bam-tag") o->bam_tag = v();
         else if (a == "--valid-chars") o->valid_chars = v();
         else if (a == "--device") o->device = atol(v().c_str());
@@ -149,6 +152,10 @@ bool parse(int argc, char** argv, Opts* o)
     if (o->vcf.empty() || o->bam.empty() || o->fasta.empty() || o->barcodes.empty()) { fprintf(stderr, "error: --vcf, --bam, --fasta and --cell-barcodes are required\n"); return false; }
     if (o->scoring != "consensus" && o->scoring != "coverage" && o->scoring != "alt_frac") { fprintf(stderr, "error: invalid --scoring-method\n"); return false; }
     if (o->bam_tag.size() != 2) { fprintf(stderr, "error: --bam-tag must have two characters\n"); return false; }
+    if (o->umi && o->collapse_mates) {
+        fprintf(stderr, "error: --collapse-mates cannot be combined with --umi (mates share their UB tag, so --umi already counts a fragment once)\n");
+        return false;
+    }
     if (o->threads < 1) o->threads = 1;
     if (o->shard_loci < 0) o->shard_loci = 0;
     if (o->devices.empty()) o->devices.push_back(int(o->device));
@@ -326,7 +333,8 @@ int main(int argc, char** argv)
                 cfg.device = cuda_index[d];
                 cfg.mode = o.scoring == "consensus" ? VTX_MODE_CONSENSUS : o.scoring == "coverage" ? VTX_MODE_COVERAGE : VTX_MODE_ALT_FRAC;
                 cfg.flags = VTX_F_VALUES_ONLY;       // the writers need row, col and the matrix values only
-                cfg.use_umi = o.umi; cfg.match = 1; cfg.mismatch = -5; cfg.gap_open = -5; cfg.gap_extend = -1; cfg.min_score = 25;
+                if (o.collapse_mates) cfg.flags |= VTX_F_NAME_KEYS;      // name keys through the UMI collapse
+                cfg.use_umi = o.umi || o.collapse_mates; cfg.match = 1; cfg.mismatch = -5; cfg.gap_open = -5; cfg.gap_extend = -1; cfg.min_score = 25;
                 cfg.band_k = 6; cfg.band_w = 20; cfg.band_mode = VTX_BAND_FULL;          // main.rs:33-34
                 if (vtx_create(&cfg, &ln.ctx) != VTX_OK) { ln.err = vtx_last_error(nullptr); return 1; }
                 if (vtx_set_barcodes(ln.ctx, bcs.bytes.data(), bcs.off.data(), uint32_t(bcs.keys.size())) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
@@ -362,7 +370,8 @@ int main(int argc, char** argv)
     StageArgs sa;
     sa.padding = o.padding; sa.mapq = uint32_t(o.mapq); sa.primary_only = o.primary; sa.no_duplicates = o.no_dups;
     sa.bam_tag[0] = o.bam_tag[0]; sa.bam_tag[1] = o.bam_tag[1];
-    sa.with_umi = o.umi || dumping;            // without --umi the engine never looks at the UB keys: they are not staged
+    sa.with_umi = o.umi || o.collapse_mates || dumping;      // without --umi the engine never looks at the UB keys: they are not staged
+    sa.name_keys = o.collapse_mates;
     for (unsigned char c : o.valid_chars) sa.valid[c] = true;
 
     // ---- staging: worker threads produce shards of `shard_loci` records; one lane per GPU consumes its range in order ----

@@ -34,6 +34,7 @@ struct StageArgs {
     char bam_tag[2] = { 'C', 'B' };
     bool valid[256] = {};        // --valid-chars
     bool with_umi = true;        // stage the UB keys (--umi, or a dump for the tests); without --umi nobody reads them
+    bool name_keys = false;      // --collapse-mates: the staged key is the QNAME (per-shard interner), not the UB tag
     // --gpu-inflate: the BGZF members of a shard's loci are inflated in one device call (vtx_bgzf_inflate) instead of one
     // by one on the staging thread; empty = host inflate
     Bgzf::BulkInflate bulk_inflate;
@@ -137,6 +138,23 @@ public:
 private:
     std::mutex mu_;
     std::unordered_map<std::string, uint64_t> map_;
+};
+
+// --collapse-mates: QNAME -> key, first-seen order, for one shard at a time.  Keys only meet inside one locus, so a table per
+// shard (owned by the staging thread) is enough; a name of "*" (SAM: no name) gets a fresh key every time.
+class NameInterner {
+public:
+    void clear() { map_.clear(); next_ = 0; }
+    uint64_t key(const uint8_t* s, uint32_t len)
+    {
+        if (len == 1 && s[0] == '*') return next_++;
+        auto it = map_.emplace(std::string(reinterpret_cast<const char*>(s), len), next_);
+        if (it.second) ++next_;
+        return it.first->second;
+    }
+private:
+    std::unordered_map<std::string, uint64_t> map_;
+    uint64_t next_ = 0;
 };
 
 // rust-htslib 0.36 CigarStringView::read_pos(p, include_softclips = false, include_dels = true) folded
@@ -326,6 +344,8 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
     }
     static thread_local ReadIndex read_index;               // record virtual offset -> staged read id (table reused across shards)
     read_index.clear();
+    static thread_local NameInterner names;                 // --collapse-mates: this shard's QNAME keys
+    names.clear();
     BamRecord rec;
     std::string ref_hap, alt_hap;
     out->cand_start.push_back(0);
@@ -384,7 +404,10 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
                         }
                     }
                     out->read_cb_key.push_back(key);
-                    if (a.with_umi) {
+                    if (a.name_keys) {
+                        n = rec.l_read_name() ? rec.l_read_name() - 1 : 0;                                    // without the NUL
+                        out->read_umi_key.push_back(names.key(rec.p + 32, n));
+                    } else if (a.with_umi) {
                         const uint8_t* ub = rec.aux_z("UB", &n);                                              // main.rs:752-757
                         out->read_umi_key.push_back(ub ? umis.key(ub, n) : VTX_NO_UMI);
                     }

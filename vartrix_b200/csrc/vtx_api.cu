@@ -99,7 +99,7 @@ struct InSlot {
 struct StageSlot {
     DBuf comp, desc, status, stream, entry, seg_count, seg_first, rec_off, rec_tid, rec_pos, rec_end, rec_fm, l_start, l_end,
         locus_row, hap, ref_off, ref_len, alt_off, alt_len, cand_count, cand_first, cand_rec, used, read_off, read_len,
-        read_cb_off, read_cb_len, read_umi, cand_start, scalars;
+        read_cb_off, read_cb_len, read_umi, cand_start, scalars, name_tab;
     cudaEvent_t staged = nullptr, free_ev = nullptr;
     bool used_once = false;
 };
@@ -1029,6 +1029,8 @@ int vtx_create(const vtx_config* cfg, vtx_ctx** out)
         return set_err(nullptr, VTX_E_UNSUPPORTED, "scoring constants are compiled in: match %d mismatch %d gap_open %d gap_extend %d (main.rs:35-38)",
                        kMatch, kMismatch, kGapOpen, kGapExtend);
     if (cfg->mode < 0 || cfg->mode > 2) return set_err(nullptr, VTX_E_INVALID, "unknown mode %d", cfg->mode);
+    if ((cfg->flags & VTX_F_NAME_KEYS) && !cfg->use_umi)
+        return set_err(nullptr, VTX_E_INVALID, "VTX_F_NAME_KEYS collapses reads through the UMI path: it needs use_umi");
     if (cfg->band_mode != VTX_BAND_FULL && cfg->band_mode != VTX_BAND_MODEL) return set_err(nullptr, VTX_E_INVALID, "unknown band_mode %d", cfg->band_mode);
     if (cfg->band_k < 0 || cfg->band_k > 8 || cfg->band_w < 0 || cfg->band_w > 4096)
         return set_err(nullptr, VTX_E_UNSUPPORTED, "band constants out of range: K %d (1..8; 0 = %d), W %d (0 = %d; main.rs:33-34)", cfg->band_k, kBandK, cfg->band_w, kBandW);
@@ -1287,7 +1289,8 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
     if (nm && (rc = launch_inflate(ctx, ss, sl.desc.p, nm, sl.comp.p, sl.stream.p, sl.status.p, d_sc, 1))) return fail_out(rc);
     stage::Params sp{};
     sp.s = P<uint8_t>(sl.stream); sp.s_len = stream_len; sp.tid = sh->tid; sp.mapq_min = sh->mapq; sp.primary_only = sh->primary_only;
-    sp.no_duplicates = sh->no_duplicates; sp.want_umi = ctx->cfg.use_umi ? 1 : 0; sp.tag0 = uint8_t(sh->bam_tag[0]); sp.tag1 = uint8_t(sh->bam_tag[1]);
+    const bool name_keys = (ctx->cfg.flags & VTX_F_NAME_KEYS) != 0;       // the keys come from vtx_k_name_key, not from UB tags
+    sp.no_duplicates = sh->no_duplicates; sp.want_umi = ctx->cfg.use_umi && !name_keys ? 1 : 0; sp.tag0 = uint8_t(sh->bam_tag[0]); sp.tag1 = uint8_t(sh->bam_tag[1]);
     // ---- record boundaries ----
     const uint32_t n_seg = ne ? ne - 1 : 0;
     ENS(sl.seg_count, size_t(n_seg + 1) * 4); ENS(sl.seg_first, size_t(n_seg + 2) * 4);
@@ -1353,8 +1356,16 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
         stage::vtx_k_read_emit<<<blocks_for(n_rec, 128), 128, 0, ss>>>(sp, n_rec, P<uint64_t>(sl.rec_off), P<uint32_t>(sl.used), P<uint64_t>(sl.read_off),
                                                                        P<uint32_t>(sl.read_len), P<uint32_t>(sl.read_cb_off), P<uint16_t>(sl.read_cb_len),
                                                                        P<uint64_t>(sl.read_umi), d_sc + 1);
+    if (name_keys && n_rec) {             // --collapse-mates: every name can be keyed here, so no wait follows
+        uint32_t tab_size = 1;
+        while (tab_size < 2 * n_rec) tab_size <<= 1;                   // n_rec < 2^28: the records of < 4 GiB of stream
+        ENS(sl.name_tab, size_t(tab_size) * 4);
+        CK(cudaMemsetAsync(sl.name_tab.p, 0xFF, size_t(tab_size) * 4, ss));
+        stage::vtx_k_name_key<<<blocks_for(n_rec, 128), 128, 0, ss>>>(sp, n_rec, P<uint64_t>(sl.rec_off), P<uint32_t>(sl.used),
+                                                                      P<uint32_t>(sl.name_tab), tab_size - 1, P<uint64_t>(sl.read_umi));
+    }
     CK(cudaGetLastError());
-    if (ctx->cfg.use_umi && n_rec) {      // wait #3 only with --umi: a UB string the device cannot key sends the shard back to the host
+    if (ctx->cfg.use_umi && !name_keys && n_rec) {      // wait #3 only with --umi: a UB string the device cannot key sends the shard back to the host
         CK(cudaMemcpyAsync(hs + 1, d_sc + 1, 4, cudaMemcpyDeviceToHost, ss));
         CK(cudaStreamSynchronize(ss));
         if (hs[1] & stage::kErrExoticUmi) return fail_out(set_err(ctx, VTX_E_UNSUPPORTED, "vtx_submit_bam: a UB tag outside vtx_pack_umi's alphabet needs the host's interner; stage this shard on the host"));

@@ -6,6 +6,7 @@
 //   fetch          every record of the contig with pos < end and bam_endpos > start, in file order   (main.rs:822-829)
 //   record filters mapq, --primary-alignments, --no-duplicates, useful_alignment, in that order      (main.rs:833-865)
 //   tags           CB (or --bam-tag) and UB: first aux field of that name, type Z                      (main.rs:737-757)
+//                  or, with --collapse-mates, the QNAME as the molecule key instead of UB (name_key below)
 // The record stream is walked from the BAI chunk starts that fall into the shard's range (record boundaries by
 // construction of the index), one thread per segment; everything after that is one thread per record or per locus.
 // Nothing is copied: reads and tag bytes are referenced inside the inflated stream.
@@ -275,6 +276,60 @@ __host__ __device__ inline void read_emit(const Params& P, uint32_t i, const uin
     }
 }
 
+// ---- 5. --collapse-mates (VTX_F_NAME_KEYS): one thread per record, the read's molecule key is its QNAME --------------------
+// Open addressing over record indices: `tab` has a power-of-two size >= 2 * n_rec and starts out all kEmptySlot.  A record walks
+// its probe chain and either claims the first empty slot (key = its own index) or meets an occupant with the same name bytes
+// (key = the occupant's index).  Slots only ever go from empty to occupied, so all records of one name walk the same chain up
+// to the first of them to claim a slot, and meet it there.  A QNAME of "*" (no name) is never inserted and keeps its own index,
+// which no occupant can hold: the keys stay injective.  Keys are compared only inside one locus, so the values do not matter.
+constexpr uint32_t kEmptySlot = 0xFFFFFFFFu;
+
+__host__ __device__ inline uint32_t claim_slot(uint32_t* p, uint32_t v)      // -> the slot's value before the call
+{
+#ifdef __CUDA_ARCH__
+    return atomicCAS(p, kEmptySlot, v);
+#else
+    const uint32_t old = *p;
+    if (old == kEmptySlot) *p = v;
+    return old;
+#endif
+}
+
+struct NameHash {                // FNV-1a over the name bytes, folded to 32 bits
+    __host__ __device__ uint32_t operator()(const uint8_t* s, uint32_t n) const
+    {
+        uint64_t h = 0xcbf29ce484222325ull;
+        for (uint32_t i = 0; i < n; ++i) { h ^= s[i]; h *= 0x100000001b3ull; }
+        return uint32_t(h ^ (h >> 32));
+    }
+};
+
+__host__ __device__ inline const uint8_t* qname_of(const uint8_t* s, const uint64_t* rec_off, uint32_t i, uint32_t* len)
+{
+    const uint8_t* b = s + rec_off[i] + 4;
+    *len = b[8] ? uint32_t(b[8]) - 1u : 0u;          // l_read_name counts the trailing NUL
+    return b + 32;
+}
+
+template <class Hash>
+__host__ __device__ inline void name_key(const Params& P, uint32_t i, const uint64_t* rec_off, const uint32_t* used, uint32_t* tab,
+                                         uint32_t tab_mask, uint64_t* read_umi, const Hash& hash)
+{
+    if (!used[i]) { read_umi[i] = kNoUmi; return; }
+    uint32_t n = 0;
+    const uint8_t* name = qname_of(P.s, rec_off, i, &n);
+    if (n == 1 && name[0] == '*') { read_umi[i] = i; return; }
+    for (uint32_t h = hash(name, n) & tab_mask;; h = (h + 1) & tab_mask) {
+        const uint32_t occ = claim_slot(&tab[h], i);
+        if (occ == kEmptySlot) { read_umi[i] = i; return; }
+        uint32_t m = 0;
+        const uint8_t* other = qname_of(P.s, rec_off, occ, &m);
+        bool same = m == n;
+        for (uint32_t k = 0; same && k < n; ++k) same = other[k] == name[k];
+        if (same) { read_umi[i] = occ; return; }
+    }
+}
+
 #ifdef __CUDACC__
 constexpr int kWalkWarps = 4, kWalkWindow = 4096;          // bytes of the stream a warp keeps in shared memory
 struct WindowFetch {
@@ -330,6 +385,13 @@ __global__ void vtx_k_read_emit(Params P, uint32_t n_rec, const uint64_t* __rest
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_rec) read_emit(P, i, rec_off, used, read_off, read_len, read_cb_off, read_cb_len, read_umi, err);
+}
+
+__global__ void vtx_k_name_key(Params P, uint32_t n_rec, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ used,
+                               uint32_t* __restrict__ tab, uint32_t tab_mask, uint64_t* __restrict__ read_umi)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_rec) name_key(P, i, rec_off, used, tab, tab_mask, read_umi, NameHash{});
 }
 
 // cand_start (u64, what the pipeline expects) from the u32 exclusive scan of the per-locus counts

@@ -375,19 +375,26 @@ class Engine:
 
     def __init__(self, scoring_method: str = "consensus", umi: bool = False, device: int = 0, stream: int = 0,
                  keep_scores: bool = False, min_score: int = 25, no_split: bool = False,
-                 values_only: bool = False, no_fold: bool = False, band_k: int = 0, band_w: int = 0, band_mode: int = 0):
+                 values_only: bool = False, no_fold: bool = False, band_k: int = 0, band_w: int = 0, band_mode: int = 0,
+                 collapse_mates: bool = False):
+        """collapse_mates: count each template once per (locus, cell) -- the reads' keys are QNAME keys and go through the
+        UMI collapse.  Host batches carry those keys in read_umi_key (the CLI's `--collapse-mates --dump-staged` writes
+        them); submit_bam interns the names on the device.  Not combinable with umi=True."""
+        if umi and collapse_mates:
+            raise ValueError("collapse_mates replaces the UB keys: it cannot be combined with umi=True")
         self._L = _capi.load()
-        cfg = _capi.Config(device=device, mode=MODES[scoring_method], use_umi=int(bool(umi)), match=1, mismatch=-5,
+        cfg = _capi.Config(device=device, mode=MODES[scoring_method], use_umi=int(bool(umi or collapse_mates)), match=1, mismatch=-5,
                            gap_open=-5, gap_extend=-1, min_score=min_score, stream=stream or None,
                            flags=(_capi.F_KEEP_SCORES if keep_scores else 0) | (_capi.F_NO_SPLIT if no_split else 0) |
-                           (_capi.F_VALUES_ONLY if values_only else 0) | (_capi.F_NO_FOLD if no_fold else 0),
+                           (_capi.F_VALUES_ONLY if values_only else 0) | (_capi.F_NO_FOLD if no_fold else 0) |
+                           (_capi.F_NAME_KEYS if collapse_mates else 0),
                            band_k=band_k, band_w=band_w, band_mode=band_mode)
         h = C.c_void_p()
         rc = self._L.vtx_create(C.byref(cfg), C.byref(h))
         if rc != 0:
             raise VtxError(f"vtx_create failed ({rc}): {self._L.vtx_last_error(None).decode()}")
         self._h = h
-        self.scoring_method, self.umi, self.device = scoring_method, umi, device
+        self.scoring_method, self.umi, self.device, self.collapse_mates = scoring_method, umi, device, collapse_mates
         self._keep = []     # host buffers that must outlive the asynchronous copies
 
     def close(self):
