@@ -276,7 +276,8 @@ int         vtx_bgzf_inflate(vtx_ctx* ctx, const vtx_bgzf_block* blocks, uint32_
  * (record boundaries), builds the haplotype windows from the FASTA -- and hands all of it over.  The device then does what
  * csrc/host/stager.hpp does on staging threads and the reference does through rust-htslib: every record of contig `tid`
  * with pos < end and bam_endpos > start per locus, in file order (main.rs:822-829); mapq / primary / duplicate /
- * useful_alignment filters in that order (main.rs:833-865); CB (`bam_tag`) and UB as the first Z-typed aux field of that
+ * useful_alignment filters in that order (main.rs:833-865), then the base-quality floor if one was set (see
+ * vtx_set_min_base_quality below); CB (`bam_tag`) and UB as the first Z-typed aux field of that
  * name (main.rs:737-757) -- with VTX_F_NAME_KEYS the QNAME instead of UB, interned on the device (a hash table of record
  * indices: key = the index of the first record with that name; "*" keeps its own index); then the same pipeline as
  * vtx_submit.  Loci must be ascending on one contig of a
@@ -317,6 +318,15 @@ typedef struct vtx_bam_metrics {
 int         vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* shard);
 /* Counters of every vtx_submit_bam since the ctx was created (waits for the staging stream). */
 int         vtx_bam_metrics_get(vtx_ctx* ctx, vtx_bam_metrics* out);
+/* --min-base-quality for every later vtx_submit_bam on this ctx (0, the default, turns it off; VTX_E_INVALID above 93).
+ * After the four record filters, a (read, locus) pair is dropped when one of its judged bases has a quality below
+ * min_q: the bases aligned to the REF span [start, end), and the bases inserted right after a reference base of that span
+ * (soft clips, deletions and skips judge nothing).  A pair without judged bases, or a record without qualities (0xFF), is
+ * kept.  Host batches (vtx_submit, vtx_submit2 and the device variants) carry no qualities: their callers apply the floor
+ * while staging, as the CLI's stager does. */
+int         vtx_set_min_base_quality(vtx_ctx* ctx, uint32_t min_q);
+/* Pairs the floor above dropped, summed over every vtx_submit_bam since the ctx was created (waits for the staging stream). */
+int         vtx_bam_low_base_quality(vtx_ctx* ctx, uint64_t* out);
 
 /* Injective code of a cell-barcode tag of the form [ACGT]{1,24}(-N)? with N = 1..99 written without a leading zero:
  * 2 bits per base, 5 bits length, 7 bits N (0 = no suffix); < 2^60.  Returns VTX_NO_CB_KEY if the bytes have another

@@ -31,6 +31,7 @@ SYMBOLS = [
     "vtx_finish_device", "vtx_fetch", "vtx_sync", "vtx_wait_copies", "vtx_score_pairs", "vtx_pack_umi", "vtx_last_timing", "vtx_last_tile_counts",
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
+    "vtx_set_min_base_quality", "vtx_bam_low_base_quality",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
 CB_EXOTIC = 0x8000000000000000
@@ -164,6 +165,10 @@ def load():
     L.vtx_submit_bam.argtypes = [C.c_void_p, C.POINTER(BamShard)]
     L.vtx_bam_metrics_get.restype = C.c_int
     L.vtx_bam_metrics_get.argtypes = [C.c_void_p, C.POINTER(BamMetrics)]
+    L.vtx_set_min_base_quality.restype = C.c_int
+    L.vtx_set_min_base_quality.argtypes = [C.c_void_p, C.c_uint32]
+    L.vtx_bam_low_base_quality.restype = C.c_int
+    L.vtx_bam_low_base_quality.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.vtx_pack_cb.restype = C.c_uint64
     L.vtx_pack_cb.argtypes = [C.c_char_p, C.c_uint32]
     L.vtx_gather_start.restype = C.c_int

@@ -48,6 +48,7 @@ struct Opts {
     std::string scoring = "consensus", bam_tag = "CB", valid_chars = "ATGCatgc", dump_staged;
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
+    uint32_t min_base_quality = 0;     // --min-base-quality (0: off)
     std::vector<int> devices;          // --devices: the loci are sharded over these GPUs (contiguous ranges, main.rs:250-254)
     bool primary = false, no_dups = false, umi = false, collapse_mates = false, ref_matrix_given = false, gpu_inflate = false, gpu_stage = false, cut_at_contigs = false;
 };
@@ -74,6 +75,8 @@ void usage()
          "      --umi                   Consider UMI information\n"
          "      --collapse-mates        Count each paired-end fragment once per cell: the records of one QNAME at a locus are\n"
          "                              collapsed like the reads of one UMI (not with --umi, which already collapses mates)\n"
+         "      --min-base-quality INT  Skip a read at a variant when a base it has there (aligned to the REF span, or\n"
+         "                              inserted right after it) has a base quality below INT, 0..93 [0: off]\n"
          "      --bam-tag TAG           BAM tag marking cells [CB]\n"
          "      --valid-chars CHARS     Valid characters in an alternative haplotype [ATGCatgc]\n"
          "      --device INT            CUDA device ordinal [0]\n"
@@ -135,6 +138,16 @@ bool parse(int argc, char** argv, Opts* o)
         else if (a == "--no-duplicates") o->no_dups = true;
         else if (a == "--umi") o->umi = true;
         else if (a == "--collapse-mates") o->collapse_mates = true;
+        else if (a == "--min-base-quality") {
+            const std::string q = v();
+            char* end = nullptr;
+            const long n = strtol(q.c_str(), &end, 10);
+            if (q.empty() || *end != 0 || n < 0 || n > long(vtx::stage::kMaxBaseQuality)) {
+                fprintf(stderr, "error: --min-base-quality must be an integer from 0 to %u, not '%s'\n", vtx::stage::kMaxBaseQuality, q.c_str());
+                return false;
+            }
+            o->min_base_quality = uint32_t(n);
+        }
         else if (a == "--bam-tag") o->bam_tag = v();
         else if (a == "--valid-chars") o->valid_chars = v();
         else if (a == "--device") o->device = atol(v().c_str());
@@ -337,6 +350,7 @@ int main(int argc, char** argv)
                 cfg.use_umi = o.umi || o.collapse_mates; cfg.match = 1; cfg.mismatch = -5; cfg.gap_open = -5; cfg.gap_extend = -1; cfg.min_score = 25;
                 cfg.band_k = 6; cfg.band_w = 20; cfg.band_mode = VTX_BAND_FULL;          // main.rs:33-34
                 if (vtx_create(&cfg, &ln.ctx) != VTX_OK) { ln.err = vtx_last_error(nullptr); return 1; }
+                if (o.min_base_quality && vtx_set_min_base_quality(ln.ctx, o.min_base_quality) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 if (vtx_set_barcodes(ln.ctx, bcs.bytes.data(), bcs.off.data(), uint32_t(bcs.keys.size())) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 if (n_dev > 1 && vtx_comm_init(ln.ctx, nccl_id, int32_t(d), int32_t(n_dev)) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 ln.ready_s = now_s();
@@ -372,6 +386,7 @@ int main(int argc, char** argv)
     sa.bam_tag[0] = o.bam_tag[0]; sa.bam_tag[1] = o.bam_tag[1];
     sa.with_umi = o.umi || o.collapse_mates || dumping;      // without --umi the engine never looks at the UB keys: they are not staged
     sa.name_keys = o.collapse_mates;
+    sa.min_base_quality = o.min_base_quality;
     for (unsigned char c : o.valid_chars) sa.valid[c] = true;
 
     // ---- staging: worker threads produce shards of `shard_loci` records; one lane per GPU consumes its range in order ----
@@ -609,6 +624,8 @@ int main(int argc, char** argv)
                 hm.num_reads += bm.num_reads; hm.num_low_mapq += bm.num_low_mapq; hm.num_non_primary += bm.num_non_primary;
                 hm.num_duplicates += bm.num_duplicates; hm.num_not_useful += bm.num_not_useful;
             }
+            uint64_t low_bq = 0;
+            if (o.min_base_quality && vtx_bam_low_base_quality(ln.ctx, &low_bq) == VTX_OK) hm.num_low_base_quality += low_bq;
             if (ln.host_fallbacks) LOG_INFO("GPU %d: %zu shard(s) staged on the host after the device declined them", ln.device, ln.host_fallbacks);
         }
     }
@@ -647,6 +664,7 @@ int main(int argc, char** argv)
     LOG_INFO("Number of alignments skipped due to being duplicates: %llu", (unsigned long long)hm.num_duplicates);
     LOG_INFO("Number of alignments skipped due to not being associated with a cell barcode: %llu", (unsigned long long)res.metrics.num_not_cell_bc);
     LOG_INFO("Number of alignments skipped due to not intersecting variant: %llu", (unsigned long long)hm.num_not_useful);
+    if (o.min_base_quality) LOG_INFO("Number of alignments skipped due to low base quality at the variant: %llu", (unsigned long long)hm.num_low_base_quality);
     LOG_INFO("Number of alignments skipped due to not having a UMI: %llu", (unsigned long long)res.metrics.num_non_umi);
     LOG_INFO("Number of VCF records skipped due to having invalid characters in the alternative haplotype: %llu", (unsigned long long)hm.num_invalid_recs);
     LOG_INFO("Number of VCF records skipped due to being multi-allelic: %llu", (unsigned long long)hm.num_multiallelic_recs);

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../../include/vartrix_b200.h"
+#include "../vtx_base_quality.cuh"
 #include "bam_reader.hpp"
 #include "inputs.hpp"
 
@@ -17,12 +18,13 @@ namespace vtxhost {
 
 struct HostMetrics {             // the host-side share of main.rs:449-459
     uint64_t num_reads = 0, num_low_mapq = 0, num_non_primary = 0, num_duplicates = 0, num_not_useful = 0,
-             num_invalid_recs = 0, num_multiallelic_recs = 0;
+             num_invalid_recs = 0, num_multiallelic_recs = 0,
+             num_low_base_quality = 0;      // --min-base-quality: not a counter of the reference
     void add(const HostMetrics& o)
     {
         num_reads += o.num_reads; num_low_mapq += o.num_low_mapq; num_non_primary += o.num_non_primary;
         num_duplicates += o.num_duplicates; num_not_useful += o.num_not_useful; num_invalid_recs += o.num_invalid_recs;
-        num_multiallelic_recs += o.num_multiallelic_recs;
+        num_multiallelic_recs += o.num_multiallelic_recs; num_low_base_quality += o.num_low_base_quality;
     }
 };
 
@@ -35,6 +37,7 @@ struct StageArgs {
     bool valid[256] = {};        // --valid-chars
     bool with_umi = true;        // stage the UB keys (--umi, or a dump for the tests); without --umi nobody reads them
     bool name_keys = false;      // --collapse-mates: the staged key is the QNAME (per-shard interner), not the UB tag
+    uint32_t min_base_quality = 0;   // --min-base-quality (0: off)
     // --gpu-inflate: the BGZF members of a shard's loci are inflated in one device call (vtx_bgzf_inflate) instead of one
     // by one on the staging thread; empty = host inflate
     Bgzf::BulkInflate bulk_inflate;
@@ -384,6 +387,9 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
                 if (a.primary_only && (fl & 0x100 || fl & 0x800)) { out->met.num_non_primary++; continue; }   // 841
                 if (a.no_duplicates && (fl & 0x400)) { out->met.num_duplicates++; continue; }                 // 849
                 if (!useful_alignment(rec, start, end)) { out->met.num_not_useful++; continue; }              // 857
+                if (a.min_base_quality && !vtx::stage::base_quality_ok(rec.p, start, end, a.min_base_quality)) {
+                    out->met.num_low_base_quality++; continue;
+                }
                 bool fresh = false;
                 const uint32_t rid = read_index.find_or_insert(rec.voff, uint32_t(out->read_len.size()), &fresh);
                 if (fresh) {

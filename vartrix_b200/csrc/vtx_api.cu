@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <array>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -126,6 +127,7 @@ struct vtx_ctx {
     uint64_t n_bam_submits = 0;
     cudaStream_t stage_stream = nullptr;
     DBuf bam_metrics;                                   // stage::LocusMetrics, cumulative
+    uint32_t min_base_quality = 0;                      // vtx_set_min_base_quality: for every later vtx_submit_bam
     DBuf stage_sums;                                    // block sums of the scans on the staging stream
     HostBuf h_stage;                                    // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
@@ -1291,6 +1293,7 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
     sp.s = P<uint8_t>(sl.stream); sp.s_len = stream_len; sp.tid = sh->tid; sp.mapq_min = sh->mapq; sp.primary_only = sh->primary_only;
     const bool name_keys = (ctx->cfg.flags & VTX_F_NAME_KEYS) != 0;       // the keys come from vtx_k_name_key, not from UB tags
     sp.no_duplicates = sh->no_duplicates; sp.want_umi = ctx->cfg.use_umi && !name_keys ? 1 : 0; sp.tag0 = uint8_t(sh->bam_tag[0]); sp.tag1 = uint8_t(sh->bam_tag[1]);
+    sp.min_base_quality = ctx->min_base_quality;
     // ---- record boundaries ----
     const uint32_t n_seg = ne ? ne - 1 : 0;
     ENS(sl.seg_count, size_t(n_seg + 1) * 4); ENS(sl.seg_first, size_t(n_seg + 2) * 4);
@@ -1372,7 +1375,8 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
     }
     if (nl) {                             // the shard is accepted: its filter counters join the running totals
         stage::LocusMetrics* d_tmp = reinterpret_cast<stage::LocusMetrics*>(sl.status.p);
-        vtx_k_add_u64<<<1, 32, 0, ss>>>(reinterpret_cast<unsigned long long*>(d_met), reinterpret_cast<const unsigned long long*>(d_tmp), 5);
+        vtx_k_add_u64<<<1, 32, 0, ss>>>(reinterpret_cast<unsigned long long*>(d_met), reinterpret_cast<const unsigned long long*>(d_tmp),
+                                        int(sizeof(stage::LocusMetrics) / 8));
     }
     CK(cudaEventRecord(sl.staged, ss));
     // ---- the usual pipeline, on the engine stream, reading reads and tags inside the stream ----
@@ -1398,8 +1402,28 @@ int vtx_bam_metrics_get(vtx_ctx* ctx, vtx_bam_metrics* out)
     memset(out, 0, sizeof(*out));
     if (!ctx->stage_stream) return VTX_OK;
     CK(cudaSetDevice(ctx->device));
-    static_assert(sizeof(vtx_bam_metrics) == sizeof(stage::LocusMetrics), "metric layouts must agree");
+    static_assert(sizeof(vtx_bam_metrics) == offsetof(stage::LocusMetrics, num_low_base_quality), "metric layouts must agree");
     CK(cudaMemcpyAsync(out, ctx->bam_metrics.p, sizeof(*out), cudaMemcpyDeviceToHost, ctx->stage_stream));
+    CK(cudaStreamSynchronize(ctx->stage_stream));
+    return VTX_OK;
+}
+
+int vtx_set_min_base_quality(vtx_ctx* ctx, uint32_t min_q)
+{
+    if (!ctx) return VTX_E_INVALID;
+    if (min_q > stage::kMaxBaseQuality) return set_err(ctx, VTX_E_INVALID, "min base quality %u out of range (0..%u)", min_q, stage::kMaxBaseQuality);
+    ctx->min_base_quality = min_q;
+    return VTX_OK;
+}
+
+int vtx_bam_low_base_quality(vtx_ctx* ctx, uint64_t* out)
+{
+    if (!ctx || !out) return VTX_E_INVALID;
+    *out = 0;
+    if (!ctx->stage_stream) return VTX_OK;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(out, static_cast<const uint8_t*>(ctx->bam_metrics.p) + offsetof(stage::LocusMetrics, num_low_base_quality), 8,
+                       cudaMemcpyDeviceToHost, ctx->stage_stream));
     CK(cudaStreamSynchronize(ctx->stage_stream));
     return VTX_OK;
 }

@@ -5,6 +5,7 @@
 // threads and the reference does through rust-htslib (vartrix src/main.rs:822-865, 737-757, 790-806):
 //   fetch          every record of the contig with pos < end and bam_endpos > start, in file order   (main.rs:822-829)
 //   record filters mapq, --primary-alignments, --no-duplicates, useful_alignment, in that order      (main.rs:833-865)
+//                  then, with --min-base-quality, the judged bases' qualities (vtx_base_quality.cuh)
 //   tags           CB (or --bam-tag) and UB: first aux field of that name, type Z                      (main.rs:737-757)
 //                  or, with --collapse-mates, the QNAME as the molecule key instead of UB (name_key below)
 // The record stream is walked from the BAI chunk starts that fall into the shard's range (record boundaries by
@@ -13,6 +14,8 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+
+#include "vtx_base_quality.cuh"
 
 namespace vtx {
 namespace stage {
@@ -27,6 +30,7 @@ struct Params {
     uint32_t mapq_min;
     int32_t primary_only, no_duplicates, want_umi;
     uint8_t tag0, tag1;          // --bam-tag
+    uint32_t min_base_quality;   // --min-base-quality (0: off)
 };
 
 // error bits (first word of `err`): the shard is then re-staged on the host, which produces the message
@@ -153,9 +157,10 @@ __host__ __device__ inline bool useful_alignment(const uint8_t* b, int64_t start
     return false;
 }
 
-struct LocusMetrics { unsigned long long num_reads, num_low_mapq, num_non_primary, num_duplicates, num_not_useful; };
+// the first five counters are vtx_bam_metrics' layout; num_low_base_quality has its own getter (vtx_bam_low_base_quality)
+struct LocusMetrics { unsigned long long num_reads, num_low_mapq, num_non_primary, num_duplicates, num_not_useful, num_low_base_quality; };
 
-// ---- 3. one thread per locus: the records it fetches, the four filters; pass 0 counts, pass 1 lists ---------------------
+// ---- 3. one thread per locus: the records it fetches, the four filters (and the base-quality floor); pass 0 counts, pass 1 lists
 __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const int64_t* l_start, const int64_t* l_end, uint32_t n_rec,
                                             const uint64_t* rec_off, const int32_t* rec_tid, const int32_t* rec_pos, const int32_t* rec_end,
                                             const uint32_t* rec_fm, const uint32_t* max_span, uint32_t* max_read, int pass, uint32_t* cand_count,
@@ -171,7 +176,7 @@ __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const i
     while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (int64_t(rec_pos[mid]) < end) lo = mid + 1; else hi = mid; }
     const uint32_t last = lo;
     uint32_t n = 0, longest = 0;
-    unsigned long long fetched = 0, low = 0, nonprim = 0, dup = 0, notuse = 0;
+    unsigned long long fetched = 0, low = 0, nonprim = 0, dup = 0, notuse = 0, lowbq = 0;
     const uint32_t base = pass ? cand_first[l] : 0;
     for (uint32_t i = first; i < last; ++i) {
         if (rec_tid[i] != P.tid || int64_t(rec_end[i]) <= start) continue;
@@ -181,6 +186,7 @@ __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const i
         if (P.primary_only && (fl & 0x900)) { ++nonprim; continue; }                      // 841
         if (P.no_duplicates && (fl & 0x400)) { ++dup; continue; }                         // 849
         if (!useful_alignment(P.s + rec_off[i] + 4, start, end)) { ++notuse; continue; }  // 857
+        if (P.min_base_quality && !base_quality_ok(P.s + rec_off[i] + 4, start, end, P.min_base_quality)) { ++lowbq; continue; }
         if (pass) { cand_rec[base + n] = i; used[i] = 1u; }
         else { const uint32_t ls = ld32(P.s + rec_off[i] + 4 + 16); if (ls > longest) longest = ls; }                       // l_seq of a read that will be scored
         ++n;
@@ -193,6 +199,7 @@ __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const i
         if (nonprim) add_u64(&met->num_non_primary, nonprim);
         if (dup) add_u64(&met->num_duplicates, dup);
         if (notuse) add_u64(&met->num_not_useful, notuse);
+        if (lowbq) add_u64(&met->num_low_base_quality, lowbq);
     }
 }
 

@@ -376,12 +376,18 @@ class Engine:
     def __init__(self, scoring_method: str = "consensus", umi: bool = False, device: int = 0, stream: int = 0,
                  keep_scores: bool = False, min_score: int = 25, no_split: bool = False,
                  values_only: bool = False, no_fold: bool = False, band_k: int = 0, band_w: int = 0, band_mode: int = 0,
-                 collapse_mates: bool = False):
+                 collapse_mates: bool = False, min_base_quality: int = 0):
         """collapse_mates: count each template once per (locus, cell) -- the reads' keys are QNAME keys and go through the
         UMI collapse.  Host batches carry those keys in read_umi_key (the CLI's `--collapse-mates --dump-staged` writes
-        them); submit_bam interns the names on the device.  Not combinable with umi=True."""
+        them); submit_bam interns the names on the device.  Not combinable with umi=True.
+        min_base_quality: submit_bam drops a (read, locus) pair when a base it has at the variant is below this quality
+        (`--min-base-quality`, 0..93, 0 = off; bam_metrics()["num_low_base_quality"] counts them).  Host batches carry no
+        qualities: the CLI's stager applies the floor to them before they are submitted."""
         if umi and collapse_mates:
             raise ValueError("collapse_mates replaces the UB keys: it cannot be combined with umi=True")
+        if not isinstance(min_base_quality, (int, np.integer)) or not 0 <= min_base_quality <= 93:
+            raise ValueError(f"min_base_quality must be an integer in 0..93, not {min_base_quality!r}")
+        min_base_quality = int(min_base_quality)
         self._L = _capi.load()
         cfg = _capi.Config(device=device, mode=MODES[scoring_method], use_umi=int(bool(umi or collapse_mates)), match=1, mismatch=-5,
                            gap_open=-5, gap_extend=-1, min_score=min_score, stream=stream or None,
@@ -395,6 +401,9 @@ class Engine:
             raise VtxError(f"vtx_create failed ({rc}): {self._L.vtx_last_error(None).decode()}")
         self._h = h
         self.scoring_method, self.umi, self.device, self.collapse_mates = scoring_method, umi, device, collapse_mates
+        self.min_base_quality = min_base_quality
+        if min_base_quality:
+            self._ck(self._L.vtx_set_min_base_quality(h, min_base_quality), "vtx_set_min_base_quality")
         self._keep = []     # host buffers that must outlive the asynchronous copies
 
     def close(self):
@@ -560,7 +569,9 @@ class Engine:
     def bam_metrics(self) -> dict:
         m = _capi.BamMetrics()
         self._ck(self._L.vtx_bam_metrics_get(self._h, C.byref(m)), "vtx_bam_metrics_get")
-        return {k: int(getattr(m, k)) for k, _ in _capi.BamMetrics._fields_}
+        low_bq = C.c_uint64()
+        self._ck(self._L.vtx_bam_low_base_quality(self._h, C.byref(low_bq)), "vtx_bam_low_base_quality")
+        return {**{k: int(getattr(m, k)) for k, _ in _capi.BamMetrics._fields_}, "num_low_base_quality": int(low_bq.value)}
 
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()

@@ -61,9 +61,12 @@ class BamWriter:
     def _voff(self):
         return (self.f.tell() << 16) | len(self.block)
 
-    def add(self, refid, pos, mapq, flag, cigar, seq: bytes, qname: bytes, aux: bytes):
-        """cigar = [(op char, len)], seq = ASCII bases."""
+    def add(self, refid, pos, mapq, flag, cigar, seq: bytes, qname: bytes, aux: bytes, qual: bytes | None = None):
+        """cigar = [(op char, len)], seq = ASCII bases, qual = one Phred value (not +33) per base; None writes absent
+        qualities (0xFF, as samtools does)."""
         l_seq = len(seq)
+        if qual is not None and len(qual) != l_seq:
+            raise ValueError(f"{len(qual)} qualities for {l_seq} bases")
         nib = bytearray((l_seq + 1) // 2)
         for i, c in enumerate(seq):
             v = _NIB.get(c, 15)
@@ -72,7 +75,7 @@ class BamWriter:
         rlen = sum(n for o, n in cigar if o in "MDN=X") if not (flag & 4) else 0
         end = pos + (rlen if rlen > 0 else 1)
         body = struct.pack("<iiBBHHHiiii", refid, pos, len(qname) + 1, mapq, reg2bin(pos, end), len(cigar), flag, l_seq, -1, -1, 0)
-        body += qname + b"\x00" + cig + bytes(nib) + b"\xff" * l_seq + aux
+        body += qname + b"\x00" + cig + bytes(nib) + (b"\xff" * l_seq if qual is None else bytes(qual)) + aux
         rec = struct.pack("<i", len(body)) + body
         if len(self.block) + len(rec) > 0xFF00:
             self._flush()
