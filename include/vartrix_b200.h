@@ -328,6 +328,41 @@ int         vtx_set_min_base_quality(vtx_ctx* ctx, uint32_t min_q);
 /* Pairs the floor above dropped, summed over every vtx_submit_bam since the ctx was created (waits for the staging stream). */
 int         vtx_bam_low_base_quality(vtx_ctx* ctx, uint64_t* out);
 
+/* ---- per-locus summary: why each matrix row holds what it holds (the CLI's --out-variant-stats) ---------------------------
+ * vtx_set_locus_stats(ctx, 1) before the first submit (VTX_E_STATE after one) makes every submit also reduce, per locus, the
+ * counters below on the device; off, the default, launches nothing extra.  After vtx_finish / vtx_finish_device,
+ * vtx_locus_stats_get hands back one entry per locus submitted since the previous finish, in submit order (shards in submit
+ * order, loci in shard order) -- ascending row when shards arrive in ascending row order, as vtx_submit asks; the library does
+ * not sort them.  Library-owned host memory, valid until the next submit or finish.  Entries are plain 32-bit counters (a shard holds fewer than 2^32
+ * candidates).  Invariants per locus:
+ *     fetched = low_mapq + non_primary + duplicate + not_useful + low_base_quality + no_cell_barcode + no_umi + scored
+ *     scored  = reads_ref + reads_alt + reads_unknown + reads_none
+ *     calls_* = reads_* without use_umi (with it: molecules after the UMI / name-key collapse, main.rs:1058-1082)
+ * The record-filter counters (fetched .. low_base_quality) are counted on the device for vtx_submit_bam shards; host batches
+ * (vtx_submit*, which only carry the survivors) leave them 0 -- their caller's stager owns them.  Every other counter comes
+ * from the device on every submit path. */
+typedef struct vtx_locus_stats {
+    uint32_t row;                 /* matrix row = VCF record index */
+    uint32_t fetched;             /* records fetch returned (main.rs:831) */
+    uint32_t low_mapq;            /* pairs dropped by each filter, counted once at the first that drops them (main.rs:833-865) */
+    uint32_t non_primary;
+    uint32_t duplicate;
+    uint32_t not_useful;
+    uint32_t low_base_quality;    /* vtx_set_min_base_quality */
+    uint32_t no_cell_barcode;     /* no tag, or a tag not in the barcode list (main.rs:867-877) */
+    uint32_t no_umi;              /* use_umi and no UB tag (main.rs:879-894) */
+    uint32_t scored;              /* pairs that reached Smith-Waterman */
+    uint32_t reads_ref, reads_alt, reads_unknown, reads_none;     /* per-pair calls (evaluate_scores, main.rs:1019-1030) */
+    uint32_t calls_ref, calls_alt, calls_unknown;                 /* the counts the matrix is built from */
+    uint32_t cells;               /* cells with at least one scored pair (the row's entries in coverage mode) */
+    uint32_t cells_ref_only;      /* consensus value 1 */
+    uint32_t cells_alt_only;      /* consensus value 2 */
+    uint32_t cells_both;          /* consensus value 3 */
+    uint32_t cells_multi_unknown; /* calls_unknown > 1 in the cell: "Check this locus manually" (main.rs:1116-1118) */
+} vtx_locus_stats;
+int         vtx_set_locus_stats(vtx_ctx* ctx, int32_t on);
+int         vtx_locus_stats_get(vtx_ctx* ctx, const vtx_locus_stats** out, uint64_t* n);
+
 /* Injective code of a cell-barcode tag of the form [ACGT]{1,24}(-N)? with N = 1..99 written without a leading zero:
  * 2 bits per base, 5 bits length, 7 bits N (0 = no suffix); < 2^60.  Returns VTX_NO_CB_KEY if the bytes have another
  * form -- the caller then lists them as an exotic tag (VTX_CB_EXOTIC | i). */

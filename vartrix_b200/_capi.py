@@ -31,7 +31,7 @@ SYMBOLS = [
     "vtx_finish_device", "vtx_fetch", "vtx_sync", "vtx_wait_copies", "vtx_score_pairs", "vtx_pack_umi", "vtx_last_timing", "vtx_last_tile_counts",
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
-    "vtx_set_min_base_quality", "vtx_bam_low_base_quality",
+    "vtx_set_min_base_quality", "vtx_bam_low_base_quality", "vtx_set_locus_stats", "vtx_locus_stats_get",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
 CB_EXOTIC = 0x8000000000000000
@@ -93,6 +93,15 @@ class BamShard(C.Structure):       # vtx_bam_shard
 class BamMetrics(C.Structure):     # vtx_bam_metrics
     _fields_ = [("num_reads", C.c_uint64), ("num_low_mapq", C.c_uint64), ("num_non_primary", C.c_uint64),
                 ("num_duplicates", C.c_uint64), ("num_not_useful", C.c_uint64)]
+
+
+LOCUS_STATS_FIELDS = ("row", "fetched", "low_mapq", "non_primary", "duplicate", "not_useful", "low_base_quality", "no_cell_barcode",
+                      "no_umi", "scored", "reads_ref", "reads_alt", "reads_unknown", "reads_none", "calls_ref", "calls_alt",
+                      "calls_unknown", "cells", "cells_ref_only", "cells_alt_only", "cells_both", "cells_multi_unknown")
+
+
+class LocusStats(C.Structure):     # vtx_locus_stats
+    _fields_ = [(f, C.c_uint32) for f in LOCUS_STATS_FIELDS]
 
 
 class Metrics(C.Structure):
@@ -169,6 +178,10 @@ def load():
     L.vtx_set_min_base_quality.argtypes = [C.c_void_p, C.c_uint32]
     L.vtx_bam_low_base_quality.restype = C.c_int
     L.vtx_bam_low_base_quality.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+    L.vtx_set_locus_stats.restype = C.c_int
+    L.vtx_set_locus_stats.argtypes = [C.c_void_p, C.c_int32]
+    L.vtx_locus_stats_get.restype = C.c_int
+    L.vtx_locus_stats_get.argtypes = [C.c_void_p, C.POINTER(C.POINTER(LocusStats)), C.POINTER(C.c_uint64)]
     L.vtx_pack_cb.restype = C.c_uint64
     L.vtx_pack_cb.argtypes = [C.c_char_p, C.c_uint32]
     L.vtx_gather_start.restype = C.c_int

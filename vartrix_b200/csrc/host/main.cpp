@@ -5,10 +5,13 @@
 #include <atomic>
 #include <condition_variable>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
+#include <cstring>
 #include <cstdlib>
 #include <malloc.h>
 #include <unistd.h>
+#include <array>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -45,7 +48,7 @@ bool exists(const std::string& p) { struct stat st; return stat(p.c_str(), &st) 
 
 struct Opts {
     std::string vcf, bam, fasta, barcodes, out_matrix = "out_matrix.mtx", ref_matrix = "ref_matrix.mtx", out_variants, out_barcodes;
-    std::string scoring = "consensus", bam_tag = "CB", valid_chars = "ATGCatgc", dump_staged;
+    std::string scoring = "consensus", bam_tag = "CB", valid_chars = "ATGCatgc", dump_staged, out_variant_stats;
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
     uint32_t min_base_quality = 0;     // --min-base-quality (0: off)
@@ -64,6 +67,8 @@ void usage()
          "  -o, --out-matrix FILE       Output Matrix Market file [out_matrix.mtx]\n"
          "      --out-variants FILE     Output variant file\n"
          "      --out-barcodes FILE     Output cell barcode file\n"
+         "      --out-variant-stats FILE  Per-variant summary table (TSV, one line per VCF record in matrix-row order): the\n"
+         "                              reads fetched, dropped by each filter and scored, their calls and the cells covered\n"
          "  -p, --padding INT           Padding on both sides of the variant [100]\n"
          "  -s, --scoring-method M      consensus | coverage | alt_frac [consensus]\n"
          "      --ref-matrix FILE       Reference matrix (coverage mode) [ref_matrix.mtx]\n"
@@ -128,6 +133,7 @@ bool parse(int argc, char** argv, Opts* o)
         else if (a == "-o" || a == "--out-matrix") o->out_matrix = v();
         else if (a == "--out-variants") o->out_variants = v();
         else if (a == "--out-barcodes") o->out_barcodes = v();
+        else if (a == "--out-variant-stats") o->out_variant_stats = v();
         else if (a == "-p" || a == "--padding") o->padding = atol(v().c_str());
         else if (a == "-s" || a == "--scoring-method") o->scoring = v();
         else if (a == "--ref-matrix") { o->ref_matrix = v(); o->ref_matrix_given = true; }
@@ -169,6 +175,10 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --collapse-mates cannot be combined with --umi (mates share their UB tag, so --umi already counts a fragment once)\n");
         return false;
     }
+    if (!o->out_variant_stats.empty() && !o->dump_staged.empty()) {
+        fprintf(stderr, "error: --out-variant-stats counts what the GPU run scores: it cannot be combined with --dump-staged\n");
+        return false;
+    }
     if (o->threads < 1) o->threads = 1;
     if (o->shard_loci < 0) o->shard_loci = 0;
     if (o->devices.empty()) o->devices.push_back(int(o->device));
@@ -189,6 +199,7 @@ void check_inputs_exist(const Opts& o)
     for (const std::string* p : { &o.fasta, &o.vcf, &o.bam, &o.barcodes })
         if (!exists(*p)) { LOG_ERR("Input file %s does not exist", p->c_str()); exit(1); }
     if (o.dump_staged.empty()) { validate_output_path(o.out_matrix); validate_output_path(o.ref_matrix); }
+    if (!o.out_variant_stats.empty()) validate_output_path(o.out_variant_stats);
     if (!exists(o.fasta + ".fai")) { LOG_ERR("File %s.fai does not exist", o.fasta.c_str()); exit(1); }
     const size_t dot = o.bam.find_last_of('.');
     const std::string ext = dot == std::string::npos ? "" : o.bam.substr(dot + 1);
@@ -287,6 +298,48 @@ void stage_into_arena(const StagedShard& s, Arena& a, vtx_batch2* b)
     for (auto& t : pool) t.join();
 }
 
+// --out-variant-stats: one line per VCF record, in matrix-row order.  `dev` holds the engine's entries of every submitted locus
+// (each row at most once over all lanes); `host_rows` / `host_filters` the stager's record-filter counters of the host-staged
+// loci, which the engine leaves 0.  Records the host never submits are multi-allelic or have an invalid ALT haplotype.
+// vtx_locus_stats is 22 u32 counters in declaration order: the writer handles an entry as that array (a copy, not a cast)
+constexpr int kStatsWords = 22;
+static_assert(sizeof(vtx_locus_stats) == kStatsWords * sizeof(uint32_t), "vtx_locus_stats: 22 counters, no padding");
+static_assert(offsetof(vtx_locus_stats, fetched) == 1 * 4 && offsetof(vtx_locus_stats, low_base_quality) == 6 * 4 &&
+              offsetof(vtx_locus_stats, scored) == 9 * 4 && offsetof(vtx_locus_stats, cells_multi_unknown) == 21 * 4,
+              "vtx_locus_stats field order");
+using StatsWords = std::array<uint32_t, kStatsWords>;      // [0] row, [1..6] fetched .. low_base_quality, [7..21] the rest
+
+bool write_variant_stats(const std::string& path, const std::vector<VcfRecord>& recs, const std::vector<vtx_locus_stats>& dev,
+                         const std::vector<uint32_t>& host_rows, const std::vector<uint32_t>& host_filters)
+{
+    std::vector<StatsWords> row(recs.size(), StatsWords{});
+    std::vector<char> submitted(recs.size(), 0);
+    for (const vtx_locus_stats& e : dev) {
+        if (e.row >= recs.size()) return false;
+        memcpy(row[e.row].data(), &e, sizeof(e));
+        submitted[e.row] = 1;
+    }
+    for (size_t i = 0; i < host_rows.size(); ++i)
+        for (int k = 0; k < 6; ++k) row[host_rows[i]][1 + k] += host_filters[i * 6 + k];     // the stager's fetched .. low_base_quality
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    fputs("variant\tchrom\tpos\tref\talt\tstatus\tfetched\tlow_mapq\tnon_primary\tduplicate\tnot_useful\tlow_base_quality\t"
+          "no_cell_barcode\tno_umi\tscored\treads_ref\treads_alt\treads_unknown\treads_none\tcalls_ref\tcalls_alt\tcalls_unknown\t"
+          "cells\tcells_ref_only\tcells_alt_only\tcells_both\tcells_multi_unknown\n", f);
+    for (size_t r = 0; r < recs.size(); ++r) {
+        const VcfRecord& v = recs[r];
+        std::string alt;
+        for (size_t k = 1; k < v.alleles.size(); ++k) { if (k > 1) alt += ','; alt += v.alleles[k]; }
+        if (v.alleles.size() == 1) alt = ".";
+        const char* status = v.alleles.size() > 2 ? "multiallelic" : submitted[r] ? "scored" : "invalid_alt";     // main.rs:646-653, 675-684
+        fprintf(f, "%s_%lld\t%s\t%lld\t%s\t%s\t%s", v.chrom.c_str(), (long long)v.pos0, v.chrom.c_str(), (long long)v.pos0 + 1,
+                v.alleles[0].c_str(), alt.c_str(), status);
+        for (int k = 1; k < kStatsWords; ++k) fprintf(f, "\t%u", row[r][k]);
+        fputc('\n', f);
+    }
+    return fclose(f) == 0;
+}
+
 }  // namespace
 
 // One GPU of the run: its own engine context, a contiguous range of shards, a thread that feeds it in order.
@@ -302,6 +355,8 @@ struct Lane {
     vtx_result dev{};                   // this lane's triplets on its device
     double ready_s = 0, wait_s = 0, submit_s = 0;      // engine up at; consumer: waiting for staged shards / inside submit calls
     Fasta fb_fa; BamFile fb_bam; bool fb_open = false; size_t host_fallbacks = 0;    // --gpu-stage: shards the device sent back
+    std::vector<vtx_locus_stats> stats;                 // --out-variant-stats: the engine's entries after this lane's finish
+    std::vector<uint32_t> host_rows, host_filters;      // ... and the stager's filter counters of the loci staged on the host
 };
 
 int main(int argc, char** argv)
@@ -351,6 +406,7 @@ int main(int argc, char** argv)
                 cfg.band_k = 6; cfg.band_w = 20; cfg.band_mode = VTX_BAND_FULL;          // main.rs:33-34
                 if (vtx_create(&cfg, &ln.ctx) != VTX_OK) { ln.err = vtx_last_error(nullptr); return 1; }
                 if (o.min_base_quality && vtx_set_min_base_quality(ln.ctx, o.min_base_quality) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
+                if (!o.out_variant_stats.empty() && vtx_set_locus_stats(ln.ctx, 1) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 if (vtx_set_barcodes(ln.ctx, bcs.bytes.data(), bcs.off.data(), uint32_t(bcs.keys.size())) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 if (n_dev > 1 && vtx_comm_init(ln.ctx, nccl_id, int32_t(d), int32_t(n_dev)) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 ln.ready_s = now_s();
@@ -387,6 +443,7 @@ int main(int argc, char** argv)
     sa.with_umi = o.umi || o.collapse_mates || dumping;      // without --umi the engine never looks at the UB keys: they are not staged
     sa.name_keys = o.collapse_mates;
     sa.min_base_quality = o.min_base_quality;
+    sa.locus_filters = !o.out_variant_stats.empty();
     for (unsigned char c : o.valid_chars) sa.valid[c] = true;
 
     // ---- staging: worker threads produce shards of `shard_loci` records; one lane per GPU consumes its range in order ----
@@ -537,6 +594,13 @@ int main(int argc, char** argv)
     for (long t = 0; t < o.threads; ++t) pool.emplace_back(worker);
 
     // one consumer per lane: shards of its range, in order, into its engine (or into the dump file)
+    auto take_stats = [&](Lane& ln) -> bool {          // --out-variant-stats: right after the lane's finish
+        if (o.out_variant_stats.empty()) return true;
+        const vtx_locus_stats* p = nullptr; uint64_t n = 0;
+        if (vtx_locus_stats_get(ln.ctx, &p, &n) != VTX_OK) return false;
+        ln.stats.assign(p, p + n);
+        return true;
+    };
     auto consume = [&](Lane& ln) {
         if (!dumping && engine_ready[size_t(ln.rank)].get() != 0) { ln.rc = 1; std::lock_guard<std::mutex> g(mu); failed = true; cv.notify_all(); return; }
         for (size_t k = ln.lo; k < ln.hi && ln.rc == 0; ++k) {
@@ -584,6 +648,10 @@ int main(int argc, char** argv)
                 ++ln.host_fallbacks;
             }
             ln.hm.add(sh->met);
+            if (!o.out_variant_stats.empty()) {
+                ln.host_rows.insert(ln.host_rows.end(), sh->locus_row.begin(), sh->locus_row.end());
+                ln.host_filters.insert(ln.host_filters.end(), sh->locus_filters.begin(), sh->locus_filters.end());
+            }
             auto recycle = [&]() { sh->clear(); std::lock_guard<std::mutex> g(mu); recycled.push_back(std::move(sh)); };
             if (dump) { dump_shard(dump, *sh); recycle(); continue; }
             Arena& ar = ln.arenas[(k - ln.lo) % 3];
@@ -600,7 +668,7 @@ int main(int argc, char** argv)
         if (dump || n_dev == 1) return;
         // several GPUs: results stay on the device; one rooted gather over NCCL brings them to lane 0 (the writer)
         vtx_result tmp{};
-        if (vtx_finish_device(ln.ctx, &ln.dev) != VTX_OK || vtx_gather_start(ln.ctx, 0) != VTX_OK || vtx_gather_wait(ln.ctx, &tmp) != VTX_OK) {
+        if (vtx_finish_device(ln.ctx, &ln.dev) != VTX_OK || !take_stats(ln) || vtx_gather_start(ln.ctx, 0) != VTX_OK || vtx_gather_wait(ln.ctx, &tmp) != VTX_OK) {
             ln.err = vtx_last_error(ln.ctx); ln.rc = 1; return;
         }
         ln.dev = tmp;
@@ -641,7 +709,7 @@ int main(int argc, char** argv)
     vtx_ctx* ctx = lanes[0].ctx;
     vtx_result res{};
     const int frc = n_dev == 1 ? vtx_finish(ctx, &res) : vtx_fetch(ctx, &lanes[0].dev, &res);
-    if (frc != VTX_OK) { printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx)); fflush(nullptr); _exit(1); }
+    if (frc != VTX_OK || (n_dev == 1 && !take_stats(lanes[0]))) { printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx)); fflush(nullptr); _exit(1); }
 
     LOG_INFO("[%.3f s] triplets on the host", now_s());
     {   // where the time went: thread-seconds of the staging pool, device milliseconds of the last finish
@@ -685,6 +753,17 @@ int main(int argc, char** argv)
         FILE* f = fopen(o.out_barcodes.c_str(), "wb");
         if (!f) { LOG_ERR("error writing barcodes file"); rc = 1; }
         else { for (const std::string& k : bcs.keys) { fwrite(k.data(), 1, k.size(), f); fputc('\n', f); } fclose(f); }
+    }
+    if (!o.out_variant_stats.empty()) {
+        validate_output_path(o.out_variant_stats);
+        std::vector<vtx_locus_stats> dev;
+        std::vector<uint32_t> host_rows, host_filters;
+        for (const Lane& ln : lanes) {
+            dev.insert(dev.end(), ln.stats.begin(), ln.stats.end());
+            host_rows.insert(host_rows.end(), ln.host_rows.begin(), ln.host_rows.end());
+            host_filters.insert(host_filters.end(), ln.host_filters.begin(), ln.host_filters.end());
+        }
+        if (!write_variant_stats(o.out_variant_stats, recs, dev, host_rows, host_filters)) { LOG_ERR("error writing variant statistics file"); rc = 1; }
     }
     LOG_INFO("[%.3f s] outputs written", now_s());
     double sum = 0;

@@ -38,6 +38,7 @@ struct StageArgs {
     bool with_umi = true;        // stage the UB keys (--umi, or a dump for the tests); without --umi nobody reads them
     bool name_keys = false;      // --collapse-mates: the staged key is the QNAME (per-shard interner), not the UB tag
     uint32_t min_base_quality = 0;   // --min-base-quality (0: off)
+    bool locus_filters = false;  // --out-variant-stats: keep the record-filter counters per locus (StagedShard::locus_filters)
     // --gpu-inflate: the BGZF members of a shard's loci are inflated in one device call (vtx_bgzf_inflate) instead of one
     // by one on the staging thread; empty = host inflate
     Bgzf::BulkInflate bulk_inflate;
@@ -88,12 +89,15 @@ struct StagedShard {
     bool identity = true;        // candidate c is read c so far (no read shared between loci)
     bool with_umi = true;        // read_umi_key is filled
     HostMetrics met;
+    // per staged locus: fetched, low mapq, non-primary, duplicate, not useful, low base quality (--out-variant-stats; the
+    // device counts the rest of vtx_locus_stats)
+    std::vector<uint32_t> locus_filters;
 
     void clear()          // keeps the capacity: shards are recycled so steady-state staging does not page-fault
     {
         locus_row.clear(); ref_off.clear(); ref_len.clear(); alt_off.clear(); alt_len.clear(); read_len.clear(); read_cb_key.clear();
         cand_read.clear(); cand_start.clear(); cb_off.clear(); read_umi_key.clear(); hap_bytes.clear();
-        read_nib.clear(); cb_bytes.clear(); met = HostMetrics(); identity = true;
+        read_nib.clear(); cb_bytes.clear(); met = HostMetrics(); identity = true; locus_filters.clear();
     }
     size_t bytes() const
     {
@@ -378,6 +382,7 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
         pad16(out->hap_bytes); out->alt_off.push_back(uint32_t(out->hap_bytes.size())); out->alt_len.push_back(uint32_t(alt_hap.size()));
         out->hap_bytes.insert(out->hap_bytes.end(), alt_hap.begin(), alt_hap.end());
 
+        const HostMetrics m0 = out->met;
         const int tid = bam.tid_of(v.chrom);
         if (tid >= 0 && bam.fetch(tid, start, end)) {                                    // main.rs:822-826
             while (bam.next(&rec)) {
@@ -424,6 +429,12 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
             if (bam.bad()) { *err = bam.error(); return false; }            // corrupt / truncated BAM: abort (main.rs:830)
         }
         out->cand_start.push_back(out->cand_read.size());
+        const HostMetrics& m1 = out->met;
+        if (a.locus_filters)
+            for (uint64_t d : { m1.num_reads - m0.num_reads, m1.num_low_mapq - m0.num_low_mapq, m1.num_non_primary - m0.num_non_primary,
+                                m1.num_duplicates - m0.num_duplicates, m1.num_not_useful - m0.num_not_useful,
+                                m1.num_low_base_quality - m0.num_low_base_quality })
+                out->locus_filters.push_back(uint32_t(d));
     }
     while (out->read_nib.size() & 3) out->read_nib.push_back(0);
     pad16(out->hap_bytes);

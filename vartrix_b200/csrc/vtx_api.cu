@@ -6,6 +6,7 @@
 #include "vtx_sw_band.cuh"
 #include "vtx_inflate.cuh"
 #include "vtx_stage.cuh"
+#include "vtx_locus_stats.cuh"
 
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
@@ -100,7 +101,7 @@ struct InSlot {
 struct StageSlot {
     DBuf comp, desc, status, stream, entry, seg_count, seg_first, rec_off, rec_tid, rec_pos, rec_end, rec_fm, l_start, l_end,
         locus_row, hap, ref_off, ref_len, alt_off, alt_len, cand_count, cand_first, cand_rec, used, read_off, read_len,
-        read_cb_off, read_cb_len, read_umi, cand_start, scalars, name_tab;
+        read_cb_off, read_cb_len, read_umi, cand_start, scalars, name_tab, lfilt;
     cudaEvent_t staged = nullptr, free_ev = nullptr;
     bool used_once = false;
 };
@@ -129,6 +130,13 @@ struct vtx_ctx {
     DBuf bam_metrics;                                   // stage::LocusMetrics, cumulative
     uint32_t min_base_quality = 0;                      // vtx_set_min_base_quality: for every later vtx_submit_bam
     DBuf stage_sums;                                    // block sums of the scans on the staging stream
+    // vtx_set_locus_stats: one vtx_locus_stats per locus submitted since the last finish (device), copied out by the finish
+    bool locus_stats = false, submitted = false;
+    DBuf lstats;
+    size_t lstats_cap = 0;                              // entries
+    uint64_t stats_n = 0, stats_last_n = 0;             // entries of the running / the last finished result set
+    HostBuf h_lstats;
+    size_t h_lstats_cap = 0;
     HostBuf h_stage;                                    // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
@@ -318,6 +326,7 @@ struct DevBatch {   // device pointers
     uint32_t class_mask = ~0u;       // tile classes that may get tiles (host batches: from the windows; device batches: all)
     uint32_t max_read_len = 0, max_hap_len = 0;
     uint64_t max_depth = ~0ull;      // most candidates of one locus (unknown for device batches: assume deep)
+    const uint32_t* lfilt = nullptr; // [n_loci][6] record-filter counters of a vtx_submit_bam shard (vtx_set_locus_stats)
 };
 
 // the allow_* switches of run_sw, shared with the host-side class mask
@@ -504,6 +513,42 @@ int grow_results(vtx_ctx* ctx, size_t need)
     return VTX_OK;
 }
 
+static_assert(sizeof(vtx_locus_stats) == sizeof(uint32_t) * lstats::kFields, "vtx_locus_stats is the kernel's record");
+
+// room for `need` entries of locus statistics; the running entries move along
+int grow_stats(vtx_ctx* ctx, size_t need)
+{
+    if (need <= ctx->lstats_cap) return VTX_OK;
+    const size_t ncap = need + need / 2 + 1024;
+    DBuf nb;
+    const cudaError_t e = cudaMalloc(&nb.p, ncap * sizeof(vtx_locus_stats));
+    if (e != cudaSuccess) { nb.p = nullptr; return set_err(ctx, VTX_E_NOMEM, "locus statistics cudaMalloc failed: %s", cudaGetErrorString(e)); }
+    nb.cap = ncap * sizeof(vtx_locus_stats);
+    if (ctx->lstats.p) {
+        if (ctx->stats_n) CK(cudaMemcpyAsync(nb.p, ctx->lstats.p, ctx->stats_n * sizeof(vtx_locus_stats), cudaMemcpyDeviceToDevice, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        CK(ctx->lstats.release());
+    }
+    ctx->lstats.swap(nb);
+    ctx->lstats_cap = ncap;
+    return VTX_OK;
+}
+
+// the per-locus reduction of this shard (vtx_locus_stats.cuh) into entries [stats_n, stats_n + n_loci); after the UMI collapse
+int launch_locus_stats(vtx_ctx* ctx, const DevBatch& b, bool have_pairs, uint64_t* launches)
+{
+    const int use_umi = ctx->cfg.use_umi ? 1 : 0;
+    lstats::Inputs in{ b.cand_start, b.cand_read, P<int32_t>(ctx->read_col), use_umi ? b.read_umi : nullptr,
+                       have_pairs ? P<uint32_t>(ctx->pair_start) : nullptr, use_umi ? P<uint32_t>(ctx->ucnt) : nullptr,
+                       P<uint32_t>(ctx->ccnt), P<uint32_t>(ctx->cslot_col), b.locus_row, b.lfilt };
+    const unsigned grid = std::min<unsigned>(b.n_loci, unsigned(ctx->n_sm) * 16);
+    lstats::vtx_k_locus_stats<<<grid, lstats::kStatsThreads, 0, ctx->stream>>>(in, b.n_loci, P<uint32_t>(ctx->lstats) + ctx->stats_n * lstats::kFields);
+    CK(cudaGetLastError());
+    ctx->stats_n += b.n_loci;
+    ++*launches;
+    return VTX_OK;
+}
+
 int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
 {
     const uint64_t nc = b.n_cand;
@@ -516,10 +561,13 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
         CK(cudaMemsetAsync(ctx->d_res_n.p, 0, 8, st));
         CK(cudaMemsetAsync(ctx->d_metrics.p, 0, 48, st));
         ctx->res_ub = 0;
+        ctx->stats_n = 0;
         ctx->finished = false;
     }
     int rc = grow_results(ctx, ctx->res_ub + nc);
     if (rc) return rc;
+    const bool stats = ctx->locus_stats && nl > 0;
+    if (stats && (rc = grow_stats(ctx, ctx->stats_n + nl))) return rc;
 
     const size_t ncp = size_t(nc) + 1;
     ENS(ctx->read_col, size_t(nr ? nr : 1) * 4);
@@ -538,7 +586,12 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
     if (nl == 0 || nc == 0) {
         if (ctx->d_cum && ctx->trec_used - 1 < kMaxCum)     // an empty shard still publishes the running triplet count
             vtx_k_bump<<<1, 32, 0, st>>>(P<unsigned long long>(ctx->d_res_n), nullptr, ctx->d_cum + (ctx->trec_used - 1));
-        CK(cudaEventRecord(tr->ev[EV_PREP], st)); CK(cudaEventRecord(tr->ev[EV_SW], st)); CK(cudaEventRecord(tr->ev[EV_POST], st));
+        CK(cudaEventRecord(tr->ev[EV_PREP], st)); CK(cudaEventRecord(tr->ev[EV_SW], st));
+        if (stats) {          // loci without candidates still get their entries (the record-filter counters, zeros elsewhere)
+            if ((rc = launch_locus_stats(ctx, b, false, &launches))) return rc;
+            tr->launches = launches;
+        }
+        CK(cudaEventRecord(tr->ev[EV_POST], st));
         ctx->timing_valid = true;
         return VTX_OK;
     }
@@ -602,6 +655,7 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
                                                                 P<uint32_t>(ctx->ucnt), P<uint32_t>(ctx->ccnt));
         ++launches;
     }
+    if (stats && (rc = launch_locus_stats(ctx, b, true, &launches))) return rc;
     vtx_k_finalize<<<blocks_for(nc, 256), 256, 0, st>>>(uint32_t(nc), n_pairs_ptr, ctx->cfg.mode, P<uint32_t>(ctx->cslot_col),
                                                         P<uint32_t>(ctx->ccnt), P<uint32_t>(ctx->keep2));
     ++launches;
@@ -952,6 +1006,7 @@ int begin_submit(vtx_ctx* ctx, const void* batch, const char* fn, const char* wh
     CK(cudaSetDevice(ctx->device));
     *tr = new_trec(ctx);
     if (!*tr) return set_err(ctx, VTX_E_CUDA, "cudaEventCreate failed");
+    ctx->submitted = true;
     return VTX_OK;
 }
 
@@ -1332,9 +1387,11 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
         ENS(sl.status, std::max<size_t>(size_t(nm) * 4 + 16, sizeof(stage::LocusMetrics) + 16));
         stage::LocusMetrics* d_tmp = reinterpret_cast<stage::LocusMetrics*>(sl.status.p);
         CK(cudaMemsetAsync(d_tmp, 0, sizeof(stage::LocusMetrics), ss));
+        if (ctx->locus_stats) ENS(sl.lfilt, size_t(nl) * lstats::kFilters * 4);
         stage::vtx_k_locus_cands<<<blocks_for(nl, 64), 64, 0, ss>>>(sp, nl, P<int64_t>(sl.l_start), P<int64_t>(sl.l_end), n_rec, P<uint64_t>(sl.rec_off),
                                                                    P<int32_t>(sl.rec_tid), P<int32_t>(sl.rec_pos), P<int32_t>(sl.rec_end), P<uint32_t>(sl.rec_fm),
-                                                                   d_sc + 2, d_sc + 3, 0, P<uint32_t>(sl.cand_count), nullptr, nullptr, nullptr, d_tmp);
+                                                                   d_sc + 2, d_sc + 3, 0, P<uint32_t>(sl.cand_count), nullptr, nullptr, nullptr, d_tmp,
+                                                                   ctx->locus_stats ? P<uint32_t>(sl.lfilt) : nullptr);
         rc = scan_u32(ctx, ss, ctx->stage_sums, P<uint32_t>(sl.cand_count), nl, P<uint32_t>(sl.cand_first), nullptr);
         if (rc) return fail_out(rc);
         CK(cudaMemcpyAsync(hs, P<uint32_t>(sl.cand_first) + nl, 4, cudaMemcpyDeviceToHost, ss));
@@ -1352,7 +1409,8 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
         stage::LocusMetrics* d_tmp = reinterpret_cast<stage::LocusMetrics*>(sl.status.p);
         stage::vtx_k_locus_cands<<<blocks_for(nl, 64), 64, 0, ss>>>(sp, nl, P<int64_t>(sl.l_start), P<int64_t>(sl.l_end), n_rec, P<uint64_t>(sl.rec_off),
                                                                    P<int32_t>(sl.rec_tid), P<int32_t>(sl.rec_pos), P<int32_t>(sl.rec_end), P<uint32_t>(sl.rec_fm),
-                                                                   d_sc + 2, d_sc + 3, 1, nullptr, P<uint32_t>(sl.cand_first), P<uint32_t>(sl.cand_rec), P<uint32_t>(sl.used), d_tmp);
+                                                                   d_sc + 2, d_sc + 3, 1, nullptr, P<uint32_t>(sl.cand_first), P<uint32_t>(sl.cand_rec), P<uint32_t>(sl.used), d_tmp,
+                                                                   nullptr);
         stage::vtx_k_widen<<<blocks_for(nl + 1, 256), 256, 0, ss>>>(nl + 1, P<uint32_t>(sl.cand_first), P<uint64_t>(sl.cand_start));
     }
     if (n_rec)
@@ -1388,6 +1446,7 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
     d.cb_bytes = P<uint8_t>(sl.stream); d.read_cb_off = P<uint32_t>(sl.read_cb_off); d.read_cb_len = P<uint16_t>(sl.read_cb_len);
     d.read_umi = ctx->cfg.use_umi ? P<uint64_t>(sl.read_umi) : nullptr; d.cand_read = P<uint32_t>(sl.cand_rec);
     d.max_read_len = max_read; d.max_hap_len = max_hap;
+    d.lfilt = ctx->locus_stats && nl ? P<uint32_t>(sl.lfilt) : nullptr;
     CK(cudaStreamWaitEvent(ctx->stream, sl.staged, 0));
     CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));
     rc = process_batch(ctx, d, tr);
@@ -1428,6 +1487,25 @@ int vtx_bam_low_base_quality(vtx_ctx* ctx, uint64_t* out)
     return VTX_OK;
 }
 
+int vtx_set_locus_stats(vtx_ctx* ctx, int32_t on)
+{
+    if (!ctx) return VTX_E_INVALID;
+    if (ctx->submitted) return set_err(ctx, VTX_E_STATE, "vtx_set_locus_stats must be called before the first submit");
+    ctx->locus_stats = on != 0;
+    return VTX_OK;
+}
+
+int vtx_locus_stats_get(vtx_ctx* ctx, const vtx_locus_stats** out, uint64_t* n)
+{
+    if (!ctx || !out || !n) return VTX_E_INVALID;
+    *out = nullptr; *n = 0;
+    if (!ctx->locus_stats) return set_err(ctx, VTX_E_STATE, "locus statistics are off: call vtx_set_locus_stats(ctx, 1) before the first submit");
+    if (!ctx->finished) return set_err(ctx, VTX_E_STATE, "vtx_locus_stats_get must follow vtx_finish / vtx_finish_device");
+    *out = ctx->stats_last_n ? ctx->h_lstats.as<const vtx_locus_stats>() : nullptr;
+    *n = ctx->stats_last_n;
+    return VTX_OK;
+}
+
 uint64_t vtx_pack_cb(const uint8_t* s, uint32_t len) { return (s || len == 0) ? pack_cb(s, len) : VTX_NO_CB_KEY; }
 
 int vtx_sync(vtx_ctx* ctx)
@@ -1452,7 +1530,19 @@ static int finish_scalars(vtx_ctx* ctx)
     uint64_t* hs = ctx->h_scalars.as<uint64_t>();
     CK(cudaMemcpyAsync(hs, ctx->d_res_n.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(hs + 1, ctx->d_metrics.p, 48, cudaMemcpyDeviceToHost, ctx->stream));
+    const uint64_t sn = ctx->finished ? 0 : ctx->stats_n;          // vtx_set_locus_stats: the entries travel with the scalars
+    if (sn) {
+        if (sn > ctx->h_lstats_cap) {
+            const size_t ncap = size_t(sn) + size_t(sn) / 4 + 1024;
+            const cudaError_t e = ctx->h_lstats.alloc(ncap * sizeof(vtx_locus_stats));
+            if (e != cudaSuccess) { ctx->h_lstats_cap = 0; return set_err(ctx, VTX_E_NOMEM, "pinned locus statistics alloc failed: %s", cudaGetErrorString(e)); }
+            ctx->h_lstats_cap = ncap;
+        }
+        CK(cudaMemcpyAsync(ctx->h_lstats.p, ctx->lstats.p, size_t(sn) * sizeof(vtx_locus_stats), cudaMemcpyDeviceToHost, ctx->stream));
+    }
     CK(cudaStreamSynchronize(ctx->stream));
+    ctx->stats_last_n = sn;
+    ctx->stats_n = 0;
     const uint64_t violated = ctx->finished ? 0 : hs[5], band_overflow = ctx->finished ? 0 : hs[6];
     ctx->last_n = ctx->finished ? 0 : hs[0];
     ctx->last_metrics.num_not_cell_bc = ctx->finished ? 0 : hs[1];

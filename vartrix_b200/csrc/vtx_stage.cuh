@@ -164,7 +164,8 @@ struct LocusMetrics { unsigned long long num_reads, num_low_mapq, num_non_primar
 __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const int64_t* l_start, const int64_t* l_end, uint32_t n_rec,
                                             const uint64_t* rec_off, const int32_t* rec_tid, const int32_t* rec_pos, const int32_t* rec_end,
                                             const uint32_t* rec_fm, const uint32_t* max_span, uint32_t* max_read, int pass, uint32_t* cand_count,
-                                            const uint32_t* cand_first, uint32_t* cand_rec, uint32_t* used, LocusMetrics* met)
+                                            const uint32_t* cand_first, uint32_t* cand_rec, uint32_t* used, LocusMetrics* met,
+                                            uint32_t* lfilt = nullptr /* pass 0, vtx_set_locus_stats: [l][6] the counters below */)
 {
     const int64_t start = l_start[l], end = l_end[l];
     // records are coordinate-sorted: candidates lie in [first pos > start - max_span, first pos >= end)
@@ -200,6 +201,10 @@ __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const i
         if (dup) add_u64(&met->num_duplicates, dup);
         if (notuse) add_u64(&met->num_not_useful, notuse);
         if (lowbq) add_u64(&met->num_low_base_quality, lowbq);
+        if (lfilt) {                     // the per-locus split of the same counters (vtx_locus_stats.cuh)
+            uint32_t* f = lfilt + size_t(l) * 6;
+            f[0] = uint32_t(fetched); f[1] = uint32_t(low); f[2] = uint32_t(nonprim); f[3] = uint32_t(dup); f[4] = uint32_t(notuse); f[5] = uint32_t(lowbq);
+        }
     }
 }
 
@@ -379,11 +384,11 @@ __global__ void vtx_k_locus_cands(Params P, uint32_t n_loci, const int64_t* __re
                                   const int32_t* __restrict__ rec_pos, const int32_t* __restrict__ rec_end, const uint32_t* __restrict__ rec_fm,
                                   const uint32_t* __restrict__ max_span, uint32_t* __restrict__ max_read, int pass, uint32_t* __restrict__ cand_count,
                                   const uint32_t* __restrict__ cand_first, uint32_t* __restrict__ cand_rec, uint32_t* __restrict__ used,
-                                  LocusMetrics* __restrict__ met)
+                                  LocusMetrics* __restrict__ met, uint32_t* __restrict__ lfilt)
 {
     const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
     if (l < n_loci) locus_cands(P, l, l_start, l_end, n_rec, rec_off, rec_tid, rec_pos, rec_end, rec_fm, max_span, max_read, pass, cand_count,
-                                cand_first, cand_rec, used, met);
+                                cand_first, cand_rec, used, met, lfilt);
 }
 __global__ void vtx_k_read_emit(Params P, uint32_t n_rec, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ used,
                                 uint64_t* __restrict__ read_off, uint32_t* __restrict__ read_len,

@@ -376,13 +376,15 @@ class Engine:
     def __init__(self, scoring_method: str = "consensus", umi: bool = False, device: int = 0, stream: int = 0,
                  keep_scores: bool = False, min_score: int = 25, no_split: bool = False,
                  values_only: bool = False, no_fold: bool = False, band_k: int = 0, band_w: int = 0, band_mode: int = 0,
-                 collapse_mates: bool = False, min_base_quality: int = 0):
+                 collapse_mates: bool = False, min_base_quality: int = 0, locus_stats: bool = False):
         """collapse_mates: count each template once per (locus, cell) -- the reads' keys are QNAME keys and go through the
         UMI collapse.  Host batches carry those keys in read_umi_key (the CLI's `--collapse-mates --dump-staged` writes
         them); submit_bam interns the names on the device.  Not combinable with umi=True.
         min_base_quality: submit_bam drops a (read, locus) pair when a base it has at the variant is below this quality
         (`--min-base-quality`, 0..93, 0 = off; bam_metrics()["num_low_base_quality"] counts them).  Host batches carry no
-        qualities: the CLI's stager applies the floor to them before they are submitted."""
+        qualities: the CLI's stager applies the floor to them before they are submitted.
+        locus_stats: every submit also sums, per locus, why its row holds what it holds; locus_stats() returns them after
+        finish() / finish_device() (vtx_set_locus_stats, include/vartrix_b200.h)."""
         if umi and collapse_mates:
             raise ValueError("collapse_mates replaces the UB keys: it cannot be combined with umi=True")
         if not isinstance(min_base_quality, (int, np.integer)) or not 0 <= min_base_quality <= 93:
@@ -404,6 +406,8 @@ class Engine:
         self.min_base_quality = min_base_quality
         if min_base_quality:
             self._ck(self._L.vtx_set_min_base_quality(h, min_base_quality), "vtx_set_min_base_quality")
+        if locus_stats:
+            self._ck(self._L.vtx_set_locus_stats(h, 1), "vtx_set_locus_stats")
         self._keep = []     # host buffers that must outlive the asynchronous copies
 
     def close(self):
@@ -572,6 +576,19 @@ class Engine:
         low_bq = C.c_uint64()
         self._ck(self._L.vtx_bam_low_base_quality(self._h, C.byref(low_bq)), "vtx_bam_low_base_quality")
         return {**{k: int(getattr(m, k)) for k, _ in _capi.BamMetrics._fields_}, "num_low_base_quality": int(low_bq.value)}
+
+    LOCUS_STATS_DTYPE = np.dtype([(f, np.uint32) for f in _capi.LOCUS_STATS_FIELDS])
+
+    def locus_stats(self) -> np.ndarray:
+        """One record per locus submitted before the last finish, in submit order (vtx_locus_stats_get): a NumPy structured
+        array with the fields of vtx_locus_stats.  Needs Engine(..., locus_stats=True)."""
+        p = C.POINTER(_capi.LocusStats)()
+        n = C.c_uint64()
+        self._ck(self._L.vtx_locus_stats_get(self._h, C.byref(p), C.byref(n)), "vtx_locus_stats_get")
+        if n.value == 0:
+            return np.zeros(0, self.LOCUS_STATS_DTYPE)
+        raw = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint32)), shape=(int(n.value) * len(_capi.LOCUS_STATS_FIELDS),))
+        return raw.copy().view(self.LOCUS_STATS_DTYPE)
 
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()
