@@ -20,11 +20,11 @@
 //               step a lane loads one pair code and its 12 substitution words (3 LDS.128), nothing to merge.
 //               The last column (H + gap, E) of every row goes to shared memory.
 //   middle      the n - 192 allele columns (9 for an SNV with --padding 100, up to 40): halves are (ref, alt)
-//               again.  Transposed wavefront: lane g owns the 19 read rows [19 g, 19 g + 19), whose (H + gap, E)
-//               start from the parked forward boundary, and walks over the columns one step per column,
-//               skewed by one column per lane; F travels down the rows (one __shfl_up per step).
-//   junction    when a lane has finished the last allele column of a haplotype it adds the parked reverse
-//               boundary of the partner rows (reversed row m - 2 - r for forward row r).
+//               again.  Lane g owns the 19 read rows [19 g, 19 g + 19), whose (H + gap, E) start from the parked
+//               forward boundary, and the 8 lanes of a unit walk over the columns together, one column per step:
+//               F down a column is a running maximum, so it crosses the lanes as one exclusive max-scan.
+//   junction    after the last allele column of a haplotype every lane adds the parked reverse boundary of the
+//               partner rows (reversed row m - 2 - r for forward row r).
 //
 // Per pair this is 2 x 96 + (n - 192) column-passes in "one read per word" units instead of 96 / 2 + (n - 96):
 // ~25 % fewer DPX instructions than vtx_k_sw_split for an SNV window.  Reads up to kFoldMaxRead bases,
@@ -118,6 +118,19 @@ __device__ __forceinline__ uint32_t fold_locate(const uint32_t* __restrict__ ts,
 constexpr int kJuncH = -2 * kGoe - kBias, kJuncE = -kGapOpen - kBias;
 constexpr uint32_t kJuncH2 = (uint32_t(uint16_t(int16_t(kJuncH - 1))) << 16) | uint32_t(uint16_t(int16_t(kJuncH)));
 constexpr uint32_t kJuncE2 = (uint32_t(uint16_t(int16_t(kJuncE - 1))) << 16) | uint32_t(uint16_t(int16_t(kJuncE)));
+
+// allele-pass constants (row c of a strip): y = a - c ge, F = P + goe + (c - 1) ge, H + goe = max(y, P + go) + goe + c ge
+static_assert(kGapExtend < 0 && kGapOpen <= 0, "the vertical gap is a running maximum only if go <= 0");
+constexpr uint32_t kFoldRowY2 = uint32_t(-kGapExtend) * 0x10001u;   // + (-ge, -ge): positive, never carries
+constexpr uint32_t kGO2 = pack2(kGapOpen, kGapOpen);                 // per-half add inside VIADDMNMX
+// P above row 0: a biased "minus infinity" that the packed adds and subtracts applied to P cannot borrow from
+constexpr uint32_t kScanNeg2 = pack2(kBias - 1024, kBias - 1024);
+// + (v, v) with v = goe + c ge < 0 onto halves >= kBias: the low half always carries exactly once (as kGoeAdd)
+__host__ __device__ constexpr uint32_t fold_row_hg_add(int c)
+{
+    return (uint32_t(uint16_t(int16_t(kGoe + c * kGapExtend - 1))) << 16) | uint32_t(uint16_t(int16_t(kGoe + c * kGapExtend)));
+}
+static_assert(fold_row_hg_add(0) == kGoeAdd, "row 0 adds plain goe");
 
 // W warps per CTA (one CTA per SM) and S slots of per-locus tables.  SHARED: the warps share the slots and
 // vtx_fold_ring.cuh hands out the tiles and slots.  Otherwise (S == W) slot w is warp w's own table and each warp takes
@@ -309,7 +322,9 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
         // =========================== middle: (ref, alt) over the allele columns, rows in registers ===========================
         {
             const int lmax = max(mid_ref, mid_alt), lmin = min(mid_ref, mid_alt);
-            const uint32_t short_mask = mid_ref < mid_alt ? 0x0000FFFFu : 0xFFFF0000u;   // half whose allele ends first
+            // the half whose allele ends first, and its last column (none for equal alleles)
+            const uint32_t short_mask = mid_ref < mid_alt ? 0x0000FFFFu : mid_alt < mid_ref ? 0xFFFF0000u : 0u;
+            const int k_short = lmin != lmax ? lmin - 1 : -1;
             uint32_t hg[R], e[R], rc[R];
             const uint8_t* cfm = cf + M + R * g;
 #pragma unroll
@@ -338,45 +353,63 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
                 }
                 best = __vmaxs2(best, (cross & mask) | (kBIAS2 & ~mask));
             };
-            // H(row above the strip, column before the first allele column) + gap: the forward boundary of that row
-            uint32_t diag_save = kGOE2;
-            if (g > 0 && R * g - 1 < mmax) diag_save = __byte_perm(row_bnd[R * g - 1].x, 0, 0x1010);
-            uint32_t hup_last = kGOE2, f_last = kNEG2;
-            const uint8_t* tab = reinterpret_cast<const uint8_t*>(midtab) - 32 * g;
-            const int steps = lmax + 7;
+            // All 8 lanes of a unit work on the same column k.  With a(r) = max(H(r-1, k-1) + s, E(r, k), 0), F runs
+            // down the column as F(r) = max(F(r-1) + ge, H(r-1) + goe), and H(r-1) = max(a(r-1), F(r-1)); the branch
+            // F(r-1) + goe never wins (go <= 0), so
+            //     F(r) = max over r' < r of a(r') + goe + (r-1-r') ge = P(r) + goe + (r-1) ge,  P(r) = max_{r' < r} y(r'),
+            // with y(r') = a(r') - r' ge.  Pass 1 computes a and y of the lane's 19 rows (y goes into hg[c], whose old
+            // value has already served as the diagonal of row c + 1); an exclusive max-scan over the unit's lanes gives
+            // P at the top of each strip; pass 2 turns y back into H + goe.  The lane keeps y relative to its first row
+            // (y(c) = a - c ge) and adds its offset -19 g ge only for the scan.  max H over a column is max a (F(r) <
+            // a(r') for some r' < r), so `best` takes a.
+            // Ranges: a is biased in [kBias, kBias + 152], y in [kBias, kBias + 152 + 151] once offset, P never below
+            // kScanNeg2 - 19 * 7: all halves stay far inside int16 and above every negative constant added to them below.
+            const uint8_t* tab = reinterpret_cast<const uint8_t*>(midtab);
 #pragma unroll kFoldMidUnroll
-            for (int s = 0; s < steps; ++s) {
-                uint32_t hup = __shfl_up_sync(0xffffffffu, hup_last, 1, 8);
-                uint32_t fup = __shfl_up_sync(0xffffffffu, f_last, 1, 8);
-                if (g == 0) { hup = kGOE2; fup = kNEG2; }
-                const int k = s - g;                                             // allele column of this lane
-                if (k >= 0 && k < lmax) {
-                    const uint8_t* trow = tab + 32 * s;                          // midtab[k][*]
-                    uint32_t diag = diag_save;
-                    diag_save = hup;
-                    uint32_t f = fup, fg = hup, hdown = hup;
-                    uint32_t hh[2];
+            for (int k = 0; k < lmax; ++k) {
+                const uint8_t* trow = tab + 32 * k;                              // midtab[k][*]
+                // H(19 g - 1, k - 1) + goe: the last row of the lane above, before pass 1 overwrites it (at k = 0 the
+                // parked forward boundary); row -1 of the matrix is H = 0
+                uint32_t diag = __shfl_up_sync(0xffffffffu, hg[R - 1], 1, 8);
+                if (g == 0) diag = kGOE2;
+                uint32_t aa[2], yy[2], ymax = kBIAS2;                            // y >= kBias: the floor changes nothing
 #pragma unroll
-                    for (int c = 0; c < R; ++c) {
-                        const uint32_t sv = *reinterpret_cast<const uint32_t*>(trow + rc[c]);
-                        const uint32_t ec = __viaddmax_s16x2(e[c], kGE2, hg[c]);          // E(r, k)
-                        f = __viaddmax_s16x2(f, kGE2, fg);                                // F(r, k)
-                        const uint32_t h = sw_h(diag, one, sv, ec, f);
-                        hh[c & 1] = h;
-                        diag = hg[c];
-                        hdown = hadd(h, one, c);
-                        fg = hdown;
-                        hg[c] = hdown;
-                        e[c] = ec;
-                        if (c & 1) best = __vimax3_s16x2(best, hh[0], hh[1]);
+                for (int c = 0; c < R; ++c) {                                    // pass 1: E, a, y
+                    const uint32_t sv = *reinterpret_cast<const uint32_t*>(trow + rc[c]);
+                    const uint32_t ec = __viaddmax_s16x2(e[c], kGE2, hg[c]);          // E(r, k)
+                    const uint32_t av = __vimax3_s16x2(diag + sv, ec, kBIAS2);       // a(r): positive add, no carry
+                    const uint32_t yv = av + kFoldRowY2 * uint32_t(c);
+                    diag = hg[c];
+                    hg[c] = yv;
+                    e[c] = ec;
+                    aa[c & 1] = av;
+                    yy[c & 1] = yv;
+                    if (c & 1) {
+                        best = __vimax3_s16x2(best, aa[0], aa[1]);
+                        ymax = __vimax3_s16x2(ymax, yy[0], yy[1]);
                     }
-                    if (R & 1) best = __vmaxs2(best, hh[0]);
-                    hup_last = hdown;
-                    f_last = f;
-                    if (k == lmin - 1 && lmin != lmax) junction(short_mask);    // the shorter allele ends here (indels only)
                 }
+                if (R & 1) {
+                    best = __vmaxs2(best, aa[0]);
+                    ymax = __vmaxs2(ymax, yy[0]);
+                }
+                // P at row 19 g: the max of y over the lanes above (shfl_up returns a lane's own value below its offset)
+                const uint32_t lane_ofs = uint32_t(-kGapExtend * R * g) * 0x10001u;
+                uint32_t p = __shfl_up_sync(0xffffffffu, ymax + lane_ofs, 1, 8);
+                if (g == 0) p = kScanNeg2;
+#pragma unroll
+                for (int o = 1; o < 8; o <<= 1) p = __vmaxs2(p, __shfl_up_sync(0xffffffffu, p, o, 8));
+                p -= lane_ofs;                                                   // halves >= 19 * 7: no borrow
+#pragma unroll
+                for (int c = 0; c < R; ++c) {                                    // pass 2: H = max(a, F), stored as H + goe
+                    const uint32_t yv = hg[c];
+                    // max(y, P + go) = H - c ge; adding goe + c ge (negative) carries exactly once from halves >= kBias
+                    hg[c] = __viaddmax_s16x2(p, kGO2, yv) + fold_row_hg_add(c);
+                    if (c + 1 < R) p = __vmaxs2(p, yv);
+                }
+                if (k == k_short) junction(short_mask);                          // the shorter allele ends here (indels only)
             }
-            junction(lmin != lmax ? ~short_mask : 0xFFFFFFFFu);                   // every lane has finished column lmax - 1
+            junction(~short_mask);                                                // every lane has finished column lmax - 1
 #pragma unroll
             for (int o = 4; o >= 1; o >>= 1) best = __vmaxs2(best, __shfl_xor_sync(0xffffffffu, best, o));
             // every lane is done with the allele table; release before the scatter, whose global atomics the release
