@@ -363,6 +363,28 @@ typedef struct vtx_locus_stats {
 int         vtx_set_locus_stats(vtx_ctx* ctx, int32_t on);
 int         vtx_locus_stats_get(vtx_ctx* ctx, const vtx_locus_stats** out, uint64_t* n);
 
+/* ---- donor log-likelihoods per cell: genotype demultiplexing of pooled cells (the CLI's --out-donors) ----------------------
+ * D donors with known genotypes, H = D + D(D-1)/2 hypotheses: h < D the singlet of donor h, then the doublets (0,1), (0,2), ...,
+ * (0,D-1), (1,2), ..., (D-2,D-1).  At a row, hypothesis h has s = g_d1 + g_d2 (a singlet d: s = 2 g_d), g the ALT dosage, and
+ * the expected ALT fraction q_s = {e, (e + 0.5)/2, 0.5, (1.5 - e)/2, 1 - e} (a doublet is a 50/50 mixture), e = error_rate.
+ * A cell with r REF and a ALT molecules at a usable row (ccnt after the UMI / name-key collapse: the counts the matrix is built
+ * from; UNKNOWN calls are not used) adds r Lr[s] + a La[s] to hypothesis h, with the int64 constants
+ * Lr[s] = llrint(log(1 - q_s) * VTX_DONOR_LL_SCALE) and La[s] = llrint(log(q_s) * VTX_DONOR_LL_SCALE).  A row is usable when every
+ * donor has a dosage there.  All sums are int64, so the result is independent of summation order, shard size and device count.
+ *
+ * vtx_set_donors: before the first submit (VTX_E_STATE after one).  dosage[row * n_donors + d] is 0, 1, 2 or VTX_GT_MISSING
+ * for rows 0 .. n_rows - 1 (the matrix rows); 2 <= n_donors <= 32 and 1e-6 <= error_rate <= 0.25, else VTX_E_INVALID.  The table
+ * is uploaded once.  Every later submit then reduces its cell slots into a per-column accumulator of
+ * n_barcodes x (H + 3) x 8 bytes on the device (420 MB at 100 000 barcodes and 32 donors), zeroed when a submit starts a
+ * fresh result set.  A locus whose row is >= n_rows is skipped and makes the next finish return VTX_E_INVALID.
+ * vtx_donor_ll_get: after vtx_finish / vtx_finish_device, the sums over the submits since the previous finish:
+ * ll[c * n_hyp + h] (int64, x VTX_DONOR_LL_SCALE) in the hypothesis order above, counts[c * 3 + {0, 1, 2}] = rows with
+ * r + a > 0, the sum of r, the sum of a.  Library-owned host memory, valid until the next submit or finish. */
+#define VTX_GT_MISSING 0xFFu
+#define VTX_DONOR_LL_SCALE 16777216      /* 2^24 */
+int         vtx_set_donors(vtx_ctx* ctx, uint32_t n_donors, uint64_t n_rows, const uint8_t* dosage, double error_rate);
+int         vtx_donor_ll_get(vtx_ctx* ctx, const int64_t** ll, const uint64_t** counts, uint32_t* n_cols, uint32_t* n_hyp);
+
 /* Injective code of a cell-barcode tag of the form [ACGT]{1,24}(-N)? with N = 1..99 written without a leading zero:
  * 2 bits per base, 5 bits length, 7 bits N (0 = no suffix); < 2^60.  Returns VTX_NO_CB_KEY if the bytes have another
  * form -- the caller then lists them as an exotic tag (VTX_CB_EXOTIC | i). */

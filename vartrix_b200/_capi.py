@@ -32,11 +32,14 @@ SYMBOLS = [
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
     "vtx_set_min_base_quality", "vtx_bam_low_base_quality", "vtx_set_locus_stats", "vtx_locus_stats_get",
+    "vtx_set_donors", "vtx_donor_ll_get",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
 CB_EXOTIC = 0x8000000000000000
 GATHER_ALL = -1
 BAND_FULL, BAND_MODEL = 0, 1
+GT_MISSING = 0xFF
+DONOR_LL_SCALE = 1 << 24
 
 
 class Config(C.Structure):
@@ -182,6 +185,11 @@ def load():
     L.vtx_set_locus_stats.argtypes = [C.c_void_p, C.c_int32]
     L.vtx_locus_stats_get.restype = C.c_int
     L.vtx_locus_stats_get.argtypes = [C.c_void_p, C.POINTER(C.POINTER(LocusStats)), C.POINTER(C.c_uint64)]
+    L.vtx_set_donors.restype = C.c_int
+    L.vtx_set_donors.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_double]
+    L.vtx_donor_ll_get.restype = C.c_int
+    L.vtx_donor_ll_get.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int64)), C.POINTER(C.POINTER(C.c_uint64)),
+                                   C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     L.vtx_pack_cb.restype = C.c_uint64
     L.vtx_pack_cb.argtypes = [C.c_char_p, C.c_uint32]
     L.vtx_gather_start.restype = C.c_int

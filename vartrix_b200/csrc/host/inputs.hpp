@@ -93,13 +93,101 @@ struct VcfRecord {
     int64_t pos0 = 0;                     // rec.pos(): 0-based
     std::vector<std::string> alleles;     // REF then ALTs; ALT "." -> only REF (main.rs:654-659)
 };
-inline bool read_vcf(const std::string& path, std::vector<VcfRecord>* out, std::string* err)
+
+// ---- genotypes of the sample columns (--out-donors): the ALT dosage of FORMAT GT ----
+constexpr uint8_t kGtMissing = 0xFF;        // VTX_GT_MISSING
+
+// One GT value -> ALT dosage: diploid a/b or a|b with alleles in {0, 1} -> the number of 1s; haploid 0 -> 0, haploid 1 -> 2;
+// anything else (a '.', an allele index >= 2, more than two alleles, an empty value) is missing.
+inline uint8_t gt_dosage(const char* s, size_t n)
+{
+    uint32_t ones = 0, alleles = 0;
+    size_t a = 0;
+    for (size_t i = 0; i <= n; ++i) {
+        if (i < n && s[i] != '/' && s[i] != '|') continue;
+        if (i - a != 1 || (s[a] != '0' && s[a] != '1')) return kGtMissing;
+        ones += s[a] == '1';
+        ++alleles;
+        a = i + 1;
+    }
+    if (alleles == 1) return uint8_t(ones * 2);
+    if (alleles == 2) return uint8_t(ones);
+    return kGtMissing;
+}
+
+struct VcfGenotypes {
+    std::vector<std::string> samples;       // the #CHROM line's columns after FORMAT, in header order
+    std::vector<uint8_t> dosage;            // [record][sample]: gt_dosage of the sample's GT subfield, or kGtMissing
+};
+
+// the record's sample columns (fields 9 ..) -> one dosage row; false when their count differs from the header's
+inline bool record_genotypes(const std::string& ln, VcfGenotypes* g)
+{
+    std::vector<std::pair<size_t, size_t>> f;       // [begin, end) of every tab-separated field
+    for (size_t p = 0;;) {
+        const size_t q = ln.find('\t', p);
+        f.emplace_back(p, q == std::string::npos ? ln.size() : q);
+        if (q == std::string::npos) break;
+        p = q + 1;
+    }
+    const size_t n_samples = f.size() > 9 ? f.size() - 9 : 0;
+    if (n_samples != g->samples.size()) return false;
+    long gt = -1;                                   // index of GT among the FORMAT keys
+    if (n_samples) {
+        long k = 0;
+        for (size_t p = f[8].first;; ++k) {
+            size_t q = ln.find(':', p);
+            if (q == std::string::npos || q > f[8].second) q = f[8].second;
+            if (q - p == 2 && ln.compare(p, 2, "GT") == 0) { gt = k; break; }
+            if (q == f[8].second) break;
+            p = q + 1;
+        }
+    }
+    for (size_t i = 0; i < n_samples; ++i) {
+        uint8_t d = kGtMissing;
+        if (gt >= 0) {
+            size_t p = f[9 + i].first;
+            const size_t e = f[9 + i].second;
+            long k = 0;
+            for (; k < gt; ++k) {                   // skip to the GT subfield
+                const size_t q = ln.find(':', p);
+                if (q == std::string::npos || q >= e) break;
+                p = q + 1;
+            }
+            if (k == gt) {
+                size_t q = ln.find(':', p);
+                if (q == std::string::npos || q > e) q = e;
+                d = gt_dosage(ln.data() + p, q - p);
+            }
+        }
+        g->dosage.push_back(d);
+    }
+    return true;
+}
+
+// `gts` (optional): also the sample names and every record's dosage row.  Without it, the sample columns are not looked at.
+inline bool read_vcf(const std::string& path, std::vector<VcfRecord>* out, std::string* err, VcfGenotypes* gts = nullptr)
 {
     std::string text;
     if (!read_text_file(path, &text, err, /*sniff_gz=*/true)) return false;
     if (text.size() >= 3 && memcmp(text.data(), "BCF", 3) == 0) { *err = "binary BCF input is not supported; convert to VCF"; return false; }
     for (auto& ln : split_lines(text)) {
+        if (gts && ln.compare(0, 6, "#CHROM") == 0) {
+            gts->samples.clear();
+            size_t p = 0;
+            for (int k = 0;; ++k) {
+                const size_t q = ln.find('\t', p);
+                if (k >= 9) gts->samples.emplace_back(ln, p, q == std::string::npos ? std::string::npos : q - p);
+                if (q == std::string::npos) break;
+                p = q + 1;
+            }
+            continue;
+        }
         if (ln.empty() || ln[0] == '#') continue;
+        if (gts && !record_genotypes(ln, gts)) {
+            *err = "malformed VCF line (its sample columns do not match the header's " + std::to_string(gts->samples.size()) + "): " + ln.substr(0, 60);
+            return false;
+        }
         std::vector<std::string> f;
         size_t p = 0;
         while (f.size() < 5) {

@@ -22,6 +22,7 @@
 #include <thread>
 
 #include "stager.hpp"
+#include "../vtx_donors.cuh"
 
 using namespace vtxhost;
 
@@ -49,6 +50,9 @@ bool exists(const std::string& p) { struct stat st; return stat(p.c_str(), &st) 
 struct Opts {
     std::string vcf, bam, fasta, barcodes, out_matrix = "out_matrix.mtx", ref_matrix = "ref_matrix.mtx", out_variants, out_barcodes;
     std::string scoring = "consensus", bam_tag = "CB", valid_chars = "ATGCatgc", dump_staged, out_variant_stats;
+    std::string out_donors, donors;            // --out-donors FILE, --donors NAME,NAME,...
+    double donor_error_rate = 0.01;            // --donor-error-rate
+    bool donor_error_rate_given = false;
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
     uint32_t min_base_quality = 0;     // --min-base-quality (0: off)
@@ -69,6 +73,10 @@ void usage()
          "      --out-barcodes FILE     Output cell barcode file\n"
          "      --out-variant-stats FILE  Per-variant summary table (TSV, one line per VCF record in matrix-row order): the\n"
          "                              reads fetched, dropped by each filter and scored, their calls and the cells covered\n"
+         "      --out-donors FILE       Assign each cell to a donor of the VCF's genotypes (TSV, one line per barcode): singlet and\n"
+         "                              doublet log-likelihoods from the cell's REF / ALT counts, the best pair and the call\n"
+         "      --donors LIST           The VCF samples that are the pool's donors, e.g. S1,S4,S2 (2 to 32) [every sample]\n"
+         "      --donor-error-rate E    Per-molecule error rate of the donor model, 1e-6 .. 0.25 [0.01]\n"
          "  -p, --padding INT           Padding on both sides of the variant [100]\n"
          "  -s, --scoring-method M      consensus | coverage | alt_frac [consensus]\n"
          "      --ref-matrix FILE       Reference matrix (coverage mode) [ref_matrix.mtx]\n"
@@ -134,6 +142,19 @@ bool parse(int argc, char** argv, Opts* o)
         else if (a == "--out-variants") o->out_variants = v();
         else if (a == "--out-barcodes") o->out_barcodes = v();
         else if (a == "--out-variant-stats") o->out_variant_stats = v();
+        else if (a == "--out-donors") o->out_donors = v();
+        else if (a == "--donors") o->donors = v();
+        else if (a == "--donor-error-rate") {
+            const std::string e = v();
+            char* end = nullptr;
+            const double x = strtod(e.c_str(), &end);
+            if (e.empty() || *end != 0 || !(x >= 1e-6 && x <= 0.25)) {
+                fprintf(stderr, "error: --donor-error-rate must be a number from 1e-6 to 0.25, not '%s'\n", e.c_str());
+                return false;
+            }
+            o->donor_error_rate = x;
+            o->donor_error_rate_given = true;
+        }
         else if (a == "-p" || a == "--padding") o->padding = atol(v().c_str());
         else if (a == "-s" || a == "--scoring-method") o->scoring = v();
         else if (a == "--ref-matrix") { o->ref_matrix = v(); o->ref_matrix_given = true; }
@@ -179,6 +200,14 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --out-variant-stats counts what the GPU run scores: it cannot be combined with --dump-staged\n");
         return false;
     }
+    if (!o->out_donors.empty() && !o->dump_staged.empty()) {
+        fprintf(stderr, "error: --out-donors sums what the GPU run counts: it cannot be combined with --dump-staged\n");
+        return false;
+    }
+    if (o->out_donors.empty() && (!o->donors.empty() || o->donor_error_rate_given)) {
+        fprintf(stderr, "error: --donors and --donor-error-rate only apply with --out-donors\n");
+        return false;
+    }
     if (o->threads < 1) o->threads = 1;
     if (o->shard_loci < 0) o->shard_loci = 0;
     if (o->devices.empty()) o->devices.push_back(int(o->device));
@@ -200,6 +229,7 @@ void check_inputs_exist(const Opts& o)
         if (!exists(*p)) { LOG_ERR("Input file %s does not exist", p->c_str()); exit(1); }
     if (o.dump_staged.empty()) { validate_output_path(o.out_matrix); validate_output_path(o.ref_matrix); }
     if (!o.out_variant_stats.empty()) validate_output_path(o.out_variant_stats);
+    if (!o.out_donors.empty()) validate_output_path(o.out_donors);
     if (!exists(o.fasta + ".fai")) { LOG_ERR("File %s.fai does not exist", o.fasta.c_str()); exit(1); }
     const size_t dot = o.bam.find_last_of('.');
     const std::string ext = dot == std::string::npos ? "" : o.bam.substr(dot + 1);
@@ -340,6 +370,87 @@ bool write_variant_stats(const std::string& path, const std::vector<VcfRecord>& 
     return fclose(f) == 0;
 }
 
+// --out-donors: the selected VCF samples, in --donors order (header order without it), and their dosage table (one row per
+// VCF record = matrix row)
+struct DonorTable {
+    std::vector<std::string> names;
+    std::vector<uint8_t> dosage;        // [record][donor]: 0..2 or kGtMissing
+    uint64_t usable = 0;                // biallelic rows where every donor has a dosage
+};
+
+bool select_donors(const std::string& list, const VcfGenotypes& g, const std::vector<VcfRecord>& recs, DonorTable* t, std::string* err)
+{
+    std::vector<size_t> idx;
+    if (list.empty()) {
+        for (size_t i = 0; i < g.samples.size(); ++i) idx.push_back(i);
+    } else {
+        for (size_t p = 0; p <= list.size();) {
+            size_t q = list.find(',', p);
+            if (q == std::string::npos) q = list.size();
+            const std::string name = list.substr(p, q - p);
+            const auto it = std::find(g.samples.begin(), g.samples.end(), name);
+            if (it == g.samples.end()) { *err = "--donors: '" + name + "' is not a sample column of the VCF"; return false; }
+            const size_t i = size_t(it - g.samples.begin());
+            if (std::find(idx.begin(), idx.end(), i) != idx.end()) { *err = "--donors: '" + name + "' is listed twice"; return false; }
+            idx.push_back(i);
+            p = q + 1;
+        }
+    }
+    if (idx.size() < vtx::donors::kMinDonors || idx.size() > vtx::donors::kMaxDonors) {
+        *err = "--out-donors needs 2 to 32 donors, not " + std::to_string(idx.size()) +
+               (list.empty() ? " (the VCF's sample columns; choose some with --donors)" : "");
+        return false;
+    }
+    const size_t ns = g.samples.size(), nd = idx.size();
+    for (const size_t i : idx) t->names.push_back(g.samples[i]);
+    t->dosage.resize(recs.size() * nd);
+    for (size_t r = 0; r < recs.size(); ++r) {
+        bool all = true;
+        for (size_t d = 0; d < nd; ++d) {
+            t->dosage[r * nd + d] = g.dosage[r * ns + idx[d]];
+            all = all && t->dosage[r * nd + d] != kGtMissing;
+        }
+        t->usable += all && recs[r].alleles.size() <= 2;
+    }
+    return true;
+}
+
+// The donor file: one line per barcode in column order.  ll [col][H] and cnt [col][3] are the engine's sums over every lane.
+// The calls use the fixed threshold T = 5 nats, compared in the integer scale.
+bool write_donors(const std::string& path, const std::vector<std::string>& barcodes, const std::vector<std::string>& names,
+                  const std::vector<int64_t>& ll, const std::vector<uint64_t>& cnt, uint64_t calls[3])
+{
+    using namespace vtx::donors;
+    const uint32_t D = uint32_t(names.size()), H = n_hyp(D);
+    const int64_t T = 5 * int64_t(kScale);
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    fputs("barcode\tvariants\tref\talt\tcall\tassignment\tsinglet_llr\tdoublet_llr\tbest_singlet\tsecond_singlet\tbest_doublet", f);
+    for (const std::string& n : names) fprintf(f, "\tll_%s", n.c_str());
+    fputc('\n', f);
+    auto pair_name = [&](uint32_t h) { uint32_t a, b; hyp_donors(h, D, &a, &b); return names[a] + "+" + names[b]; };
+    for (size_t c = 0; c < barcodes.size(); ++c) {
+        const int64_t* L = ll.data() + c * H;
+        const uint64_t* n = cnt.data() + c * 3;
+        uint32_t best = 0, pair = D;
+        for (uint32_t h = 1; h < D; ++h) if (L[h] > L[best]) best = h;
+        uint32_t second = best == 0 ? 1 : 0;            // ties go to the lowest index: strictly larger replaces
+        for (uint32_t h = second + 1; h < D; ++h) if (h != best && L[h] > L[second]) second = h;
+        for (uint32_t h = D + 1; h < H; ++h) if (L[h] > L[pair]) pair = h;
+        const int64_t s_llr = L[best] - L[second], d_llr = L[pair] - L[best];
+        const int call = n[0] == 0 ? 2 : d_llr >= T ? 1 : s_llr >= T ? 0 : 2;        // singlet, doublet, unassigned
+        ++calls[call];
+        const std::string assignment = call == 0 ? names[best] : call == 1 ? pair_name(pair) : ".";
+        fprintf(f, "%s\t%llu\t%llu\t%llu\t%s\t%s\t%.6f\t%.6f\t%s\t%s\t%s", barcodes[c].c_str(), (unsigned long long)n[0],
+                (unsigned long long)n[1], (unsigned long long)n[2], call == 0 ? "singlet" : call == 1 ? "doublet" : "unassigned",
+                assignment.c_str(), double(s_llr) / kScale, double(d_llr) / kScale, names[best].c_str(), names[second].c_str(),
+                pair_name(pair).c_str());
+        for (uint32_t d = 0; d < D; ++d) fprintf(f, "\t%.6f", double(L[d]) / kScale);
+        fputc('\n', f);
+    }
+    return fclose(f) == 0;
+}
+
 }  // namespace
 
 // One GPU of the run: its own engine context, a contiguous range of shards, a thread that feeds it in order.
@@ -357,6 +468,8 @@ struct Lane {
     Fasta fb_fa; BamFile fb_bam; bool fb_open = false; size_t host_fallbacks = 0;    // --gpu-stage: shards the device sent back
     std::vector<vtx_locus_stats> stats;                 // --out-variant-stats: the engine's entries after this lane's finish
     std::vector<uint32_t> host_rows, host_filters;      // ... and the stager's filter counters of the loci staged on the host
+    std::vector<int64_t> donor_ll;                      // --out-donors: this lane's sums after its finish
+    std::vector<uint64_t> donor_cnt;
 };
 
 int main(int argc, char** argv)
@@ -385,6 +498,16 @@ int main(int argc, char** argv)
     if (!load_barcodes(o.barcodes, &bcs, &err)) { LOG_ERR("%s", err.c_str()); return 1; }
     LOG_INFO("Loaded %zu barcodes", bcs.keys.size());
 
+    // --out-donors: the VCF (with its sample columns) is read before any GPU work, so that a bad donor list is refused first
+    std::vector<VcfRecord> recs;
+    const bool with_donors = !o.out_donors.empty();
+    DonorTable donors;
+    if (with_donors) {
+        VcfGenotypes gts;
+        if (!read_vcf(o.vcf, &recs, &err, &gts)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
+        if (!select_donors(o.donors, gts, recs, &donors, &err)) { fprintf(stderr, "error: %s\n", err.c_str()); return 1; }
+    }
+
     // CUDA context creation takes ~1 s per device: start it now, in the background, while the VCF is parsed and the
     // first shards are staged.  With several devices every lane also joins the engine's NCCL communicator.
     const size_t n_dev = dumping ? 1 : o.devices.size();
@@ -407,6 +530,9 @@ int main(int argc, char** argv)
                 if (vtx_create(&cfg, &ln.ctx) != VTX_OK) { ln.err = vtx_last_error(nullptr); return 1; }
                 if (o.min_base_quality && vtx_set_min_base_quality(ln.ctx, o.min_base_quality) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 if (!o.out_variant_stats.empty() && vtx_set_locus_stats(ln.ctx, 1) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
+                if (with_donors && vtx_set_donors(ln.ctx, uint32_t(donors.names.size()), recs.size(), donors.dosage.data(), o.donor_error_rate) != VTX_OK) {
+                    ln.err = vtx_last_error(ln.ctx); return 1;
+                }
                 if (vtx_set_barcodes(ln.ctx, bcs.bytes.data(), bcs.off.data(), uint32_t(bcs.keys.size())) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 if (n_dev > 1 && vtx_comm_init(ln.ctx, nccl_id, int32_t(d), int32_t(n_dev)) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 ln.ready_s = now_s();
@@ -415,8 +541,7 @@ int main(int argc, char** argv)
         }
     }
 
-    std::vector<VcfRecord> recs;
-    if (!read_vcf(o.vcf, &recs, &err)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
+    if (!with_donors && !read_vcf(o.vcf, &recs, &err)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
     if (recs.empty()) LOG_ERR("Warning! Zero variants found in input VCF. Output matrices will be by definition empty but will still be generated.");
     LOG_INFO("Initialized a %zu variants x %zu cell barcodes matrix", recs.size(), bcs.keys.size());
     LOG_INFO("[%.3f s] inputs parsed", now_s());
@@ -601,6 +726,14 @@ int main(int argc, char** argv)
         ln.stats.assign(p, p + n);
         return true;
     };
+    auto take_donors = [&](Lane& ln) -> bool {         // --out-donors: right after the lane's finish
+        if (!with_donors) return true;
+        const int64_t* ll = nullptr; const uint64_t* cnt = nullptr; uint32_t nc = 0, nh = 0;
+        if (vtx_donor_ll_get(ln.ctx, &ll, &cnt, &nc, &nh) != VTX_OK) return false;
+        ln.donor_ll.assign(ll, ll + size_t(nc) * nh);
+        ln.donor_cnt.assign(cnt, cnt + size_t(nc) * 3);
+        return true;
+    };
     auto consume = [&](Lane& ln) {
         if (!dumping && engine_ready[size_t(ln.rank)].get() != 0) { ln.rc = 1; std::lock_guard<std::mutex> g(mu); failed = true; cv.notify_all(); return; }
         for (size_t k = ln.lo; k < ln.hi && ln.rc == 0; ++k) {
@@ -668,7 +801,7 @@ int main(int argc, char** argv)
         if (dump || n_dev == 1) return;
         // several GPUs: results stay on the device; one rooted gather over NCCL brings them to lane 0 (the writer)
         vtx_result tmp{};
-        if (vtx_finish_device(ln.ctx, &ln.dev) != VTX_OK || !take_stats(ln) || vtx_gather_start(ln.ctx, 0) != VTX_OK || vtx_gather_wait(ln.ctx, &tmp) != VTX_OK) {
+        if (vtx_finish_device(ln.ctx, &ln.dev) != VTX_OK || !take_stats(ln) || !take_donors(ln) || vtx_gather_start(ln.ctx, 0) != VTX_OK || vtx_gather_wait(ln.ctx, &tmp) != VTX_OK) {
             ln.err = vtx_last_error(ln.ctx); ln.rc = 1; return;
         }
         ln.dev = tmp;
@@ -709,7 +842,7 @@ int main(int argc, char** argv)
     vtx_ctx* ctx = lanes[0].ctx;
     vtx_result res{};
     const int frc = n_dev == 1 ? vtx_finish(ctx, &res) : vtx_fetch(ctx, &lanes[0].dev, &res);
-    if (frc != VTX_OK || (n_dev == 1 && !take_stats(lanes[0]))) { printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx)); fflush(nullptr); _exit(1); }
+    if (frc != VTX_OK || (n_dev == 1 && (!take_stats(lanes[0]) || !take_donors(lanes[0])))) { printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx)); fflush(nullptr); _exit(1); }
 
     LOG_INFO("[%.3f s] triplets on the host", now_s());
     {   // where the time went: thread-seconds of the staging pool, device milliseconds of the last finish
@@ -764,6 +897,24 @@ int main(int argc, char** argv)
             host_filters.insert(host_filters.end(), ln.host_filters.begin(), ln.host_filters.end());
         }
         if (!write_variant_stats(o.out_variant_stats, recs, dev, host_rows, host_filters)) { LOG_ERR("error writing variant statistics file"); rc = 1; }
+    }
+    if (with_donors) {                  // the lanes' int64 sums add up to the one-GPU sums exactly
+        validate_output_path(o.out_donors);
+        const size_t H = vtx::donors::n_hyp(uint32_t(donors.names.size()));
+        std::vector<int64_t> ll(bcs.keys.size() * H, 0);
+        std::vector<uint64_t> cnt(bcs.keys.size() * 3, 0);
+        for (const Lane& ln : lanes) {
+            if (ln.donor_ll.size() != ll.size() || ln.donor_cnt.size() != cnt.size()) { LOG_ERR("donor sums of GPU %d have the wrong size", ln.device); rc = 1; continue; }
+            for (size_t i = 0; i < ll.size(); ++i) ll[i] += ln.donor_ll[i];
+            for (size_t i = 0; i < cnt.size(); ++i) cnt[i] += ln.donor_cnt[i];
+        }
+        uint64_t calls[3] = { 0, 0, 0 };
+        if (!write_donors(o.out_donors, bcs.keys, donors.names, ll, cnt, calls)) { LOG_ERR("error writing donor file"); rc = 1; }
+        std::string list;
+        for (const std::string& n : donors.names) list += (list.empty() ? "" : ",") + n;
+        LOG_INFO("Donors: %zu (%s), error rate %g; rows with a genotype for every donor: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
+                 donors.names.size(), list.c_str(), o.donor_error_rate, (unsigned long long)donors.usable, recs.size(),
+                 (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
     }
     LOG_INFO("[%.3f s] outputs written", now_s());
     double sum = 0;

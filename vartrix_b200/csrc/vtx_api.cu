@@ -7,6 +7,7 @@
 #include "vtx_inflate.cuh"
 #include "vtx_stage.cuh"
 #include "vtx_locus_stats.cuh"
+#include "vtx_donors.cuh"
 
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
@@ -137,6 +138,16 @@ struct vtx_ctx {
     uint64_t stats_n = 0, stats_last_n = 0;             // entries of the running / the last finished result set
     HostBuf h_lstats;
     size_t h_lstats_cap = 0;
+    // vtx_set_donors: the dosage table and, per column, H int64 log-likelihoods + 3 counters (then one u64 of rows outside the
+    // table), summed over the submits since the last finish; the finish copies them to h_donor
+    bool donors = false;
+    uint32_t n_donors = 0, donor_cols = 0, donor_last_cols = 0;
+    uint64_t donor_rows = 0;
+    donors::Tables donor_tab{};
+    DBuf donor_dosage, donor_usable, donor_acc, donor_count, donor_start, donor_list;
+    HostBuf h_donor;
+    size_t h_donor_cap = 0;                             // bytes
+    bool donor_valid = false;                           // h_donor holds the last finished result set
     HostBuf h_stage;                                    // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
@@ -549,6 +560,49 @@ int launch_locus_stats(vtx_ctx* ctx, const DevBatch& b, bool have_pairs, uint64_
     return VTX_OK;
 }
 
+// the donor accumulator of `cols` columns: H int64 log-likelihoods per column, then 3 u64 counters per column, then the count
+// of loci whose row lies outside the dosage table
+size_t donor_acc_bytes(uint32_t cols, uint32_t n_hyp) { return size_t(cols) * (size_t(n_hyp) + 3) * 8 + 8; }
+
+// vtx_donors.cuh on this shard's cell slots (slot indices < n_slots_ub, *n_slots of them); after the UMI collapse
+int launch_donors(vtx_ctx* ctx, const DevBatch& b, uint32_t n_slots_ub, const uint32_t* n_slots, uint64_t* launches)
+{
+    using namespace donors;
+    cudaStream_t st = ctx->stream;
+    const uint32_t H = n_hyp(ctx->n_donors), nc = ctx->donor_cols;
+    Inputs in{ P<uint32_t>(ctx->cslot_col), P<uint32_t>(ctx->cslot_locus), b.locus_row, P<uint32_t>(ctx->ccnt),
+               P<uint8_t>(ctx->donor_dosage), P<uint8_t>(ctx->donor_usable), ctx->donor_rows, nc, ctx->n_donors, H, ctx->donor_tab };
+    int64_t* ll = P<int64_t>(ctx->donor_acc);
+    uint64_t* cnt = reinterpret_cast<uint64_t*>(ll + size_t(nc) * H);
+    unsigned long long* bad = reinterpret_cast<unsigned long long*>(cnt + size_t(nc) * 3);
+    const unsigned grid = std::max(1u, std::min(blocks_for(std::max<uint64_t>(n_slots_ub, b.n_loci), kDonorThreads), unsigned(ctx->n_sm) * 16));
+    ENS(ctx->donor_count, (size_t(nc) + 1) * 4);
+    CK(cudaMemsetAsync(ctx->donor_count.p, 0, size_t(nc) * 4, st));
+    vtx_k_donor_count<<<grid, kDonorThreads, 0, st>>>(in, n_slots_ub, n_slots, b.n_loci, P<uint32_t>(ctx->donor_count), bad);
+    CK(cudaGetLastError());
+    ++*launches;
+    if (!n_slots) return VTX_OK;
+    ENS(ctx->donor_start, (size_t(nc) + 1) * 4);
+    ENS(ctx->donor_list, size_t(n_slots_ub) * 4 + 4);
+    int rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->donor_count), nc, P<uint32_t>(ctx->donor_start), launches);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(ctx->donor_count.p, 0, size_t(nc) * 4, st));
+    vtx_k_donor_scatter<<<grid, kDonorThreads, 0, st>>>(in, n_slots_ub, n_slots, P<uint32_t>(ctx->donor_start),
+                                                        P<uint32_t>(ctx->donor_count), P<uint32_t>(ctx->donor_list));
+    // one warp per column; KH = ceil(H / 32) accumulators per lane, from the instantiations below
+    const unsigned ll_grid = std::max(1u, std::min(blocks_for(uint64_t(nc) * 32, kDonorThreads), unsigned(ctx->n_sm) * 8));
+    const uint32_t* cs = P<uint32_t>(ctx->donor_start);
+    const uint32_t* lst = P<uint32_t>(ctx->donor_list);
+    if (H <= 32) vtx_k_donor_ll<1><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
+    else if (H <= 64) vtx_k_donor_ll<2><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
+    else if (H <= 160) vtx_k_donor_ll<5><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
+    else if (H <= 288) vtx_k_donor_ll<9><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
+    else vtx_k_donor_ll<17><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
+    CK(cudaGetLastError());
+    *launches += 2;
+    return VTX_OK;
+}
+
 int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
 {
     const uint64_t nc = b.n_cand;
@@ -562,12 +616,19 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
         CK(cudaMemsetAsync(ctx->d_metrics.p, 0, 48, st));
         ctx->res_ub = 0;
         ctx->stats_n = 0;
+        if (ctx->donors) {
+            ctx->donor_cols = ctx->n_barcodes;
+            const size_t bytes = donor_acc_bytes(ctx->donor_cols, donors::n_hyp(ctx->n_donors));
+            ENS(ctx->donor_acc, bytes);
+            CK(cudaMemsetAsync(ctx->donor_acc.p, 0, bytes, st));
+        }
         ctx->finished = false;
     }
     int rc = grow_results(ctx, ctx->res_ub + nc);
     if (rc) return rc;
     const bool stats = ctx->locus_stats && nl > 0;
     if (stats && (rc = grow_stats(ctx, ctx->stats_n + nl))) return rc;
+    const bool donor = ctx->donors && nl > 0;
 
     const size_t ncp = size_t(nc) + 1;
     ENS(ctx->read_col, size_t(nr ? nr : 1) * 4);
@@ -589,6 +650,10 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
         CK(cudaEventRecord(tr->ev[EV_PREP], st)); CK(cudaEventRecord(tr->ev[EV_SW], st));
         if (stats) {          // loci without candidates still get their entries (the record-filter counters, zeros elsewhere)
             if ((rc = launch_locus_stats(ctx, b, false, &launches))) return rc;
+            tr->launches = launches;
+        }
+        if (donor) {          // no slots, but the loci's rows are still checked against the table
+            if ((rc = launch_donors(ctx, b, 0, nullptr, &launches))) return rc;
             tr->launches = launches;
         }
         CK(cudaEventRecord(tr->ev[EV_POST], st));
@@ -656,6 +721,7 @@ int process_batch(vtx_ctx* ctx, const DevBatch& b, TimeRec* tr)
         ++launches;
     }
     if (stats && (rc = launch_locus_stats(ctx, b, true, &launches))) return rc;
+    if (donor && (rc = launch_donors(ctx, b, uint32_t(nc), n_pairs_ptr, &launches))) return rc;
     vtx_k_finalize<<<blocks_for(nc, 256), 256, 0, st>>>(uint32_t(nc), n_pairs_ptr, ctx->cfg.mode, P<uint32_t>(ctx->cslot_col),
                                                         P<uint32_t>(ctx->ccnt), P<uint32_t>(ctx->keep2));
     ++launches;
@@ -1506,6 +1572,50 @@ int vtx_locus_stats_get(vtx_ctx* ctx, const vtx_locus_stats** out, uint64_t* n)
     return VTX_OK;
 }
 
+int vtx_set_donors(vtx_ctx* ctx, uint32_t n_donors, uint64_t n_rows, const uint8_t* dosage, double error_rate)
+{
+    using namespace donors;
+    if (!ctx) return VTX_E_INVALID;
+    if (ctx->submitted) return set_err(ctx, VTX_E_STATE, "vtx_set_donors must be called before the first submit");
+    if (n_donors < kMinDonors || n_donors > kMaxDonors)
+        return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: %u donors; 2 to 32 are supported", n_donors);
+    if (!(error_rate >= 1e-6 && error_rate <= 0.25))
+        return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: error rate %g outside [1e-6, 0.25]", error_rate);
+    if (n_rows && !dosage) return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: dosage is NULL");
+    const size_t cells = size_t(n_rows) * n_donors;
+    std::vector<uint8_t> usable(size_t(n_rows) + 1, 0);
+    for (size_t i = 0; i < cells; ++i)
+        if (dosage[i] > 2 && dosage[i] != kMissing)
+            return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: dosage %u at row %zu, donor %zu (0, 1, 2 or VTX_GT_MISSING)",
+                           unsigned(dosage[i]), i / n_donors, i % n_donors);
+    for (uint64_t r = 0; r < n_rows; ++r) usable[r] = row_usable(dosage + size_t(r) * n_donors, n_donors) ? 1 : 0;
+    CK(cudaSetDevice(ctx->device));
+    ENS(ctx->donor_dosage, cells + 16);
+    ENS(ctx->donor_usable, usable.size());
+    if (cells) CK(cudaMemcpy(ctx->donor_dosage.p, dosage, cells, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(ctx->donor_usable.p, usable.data(), usable.size(), cudaMemcpyHostToDevice));
+    ctx->n_donors = n_donors;
+    ctx->donor_rows = n_rows;
+    ctx->donor_tab = make_tables(error_rate);
+    ctx->donors = true;
+    ctx->donor_valid = false;
+    return VTX_OK;
+}
+
+int vtx_donor_ll_get(vtx_ctx* ctx, const int64_t** ll, const uint64_t** counts, uint32_t* n_cols, uint32_t* n_hyp)
+{
+    if (!ctx || !ll || !counts || !n_cols || !n_hyp) return VTX_E_INVALID;
+    *ll = nullptr; *counts = nullptr; *n_cols = 0; *n_hyp = 0;
+    if (!ctx->donors) return set_err(ctx, VTX_E_STATE, "no donors: call vtx_set_donors before the first submit");
+    if (!ctx->finished || !ctx->donor_valid) return set_err(ctx, VTX_E_STATE, "vtx_donor_ll_get must follow vtx_finish / vtx_finish_device");
+    const uint32_t H = donors::n_hyp(ctx->n_donors);
+    *ll = ctx->h_donor.as<const int64_t>();
+    *counts = reinterpret_cast<const uint64_t*>(*ll + size_t(ctx->donor_last_cols) * H);
+    *n_cols = ctx->donor_last_cols;
+    *n_hyp = H;
+    return VTX_OK;
+}
+
 uint64_t vtx_pack_cb(const uint8_t* s, uint32_t len) { return (s || len == 0) ? pack_cb(s, len) : VTX_NO_CB_KEY; }
 
 int vtx_sync(vtx_ctx* ctx)
@@ -1540,6 +1650,23 @@ static int finish_scalars(vtx_ctx* ctx)
         }
         CK(cudaMemcpyAsync(ctx->h_lstats.p, ctx->lstats.p, size_t(sn) * sizeof(vtx_locus_stats), cudaMemcpyDeviceToHost, ctx->stream));
     }
+    uint64_t donor_bad = 0;
+    if (ctx->donors) {          // vtx_set_donors: the accumulator travels with the scalars too (zeros when nothing was submitted)
+        const uint32_t cols = ctx->finished ? ctx->n_barcodes : ctx->donor_cols;
+        const size_t bytes = donor_acc_bytes(cols, donors::n_hyp(ctx->n_donors));
+        if (bytes > ctx->h_donor_cap) {
+            ctx->donor_valid = false;
+            const cudaError_t e = ctx->h_donor.alloc(bytes);
+            if (e != cudaSuccess) { ctx->h_donor_cap = 0; return set_err(ctx, VTX_E_NOMEM, "pinned donor log-likelihood alloc failed: %s", cudaGetErrorString(e)); }
+            ctx->h_donor_cap = bytes;
+        }
+        if (ctx->finished) memset(ctx->h_donor.p, 0, bytes);
+        else CK(cudaMemcpyAsync(ctx->h_donor.p, ctx->donor_acc.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        memcpy(&donor_bad, ctx->h_donor.as<uint8_t>() + bytes - 8, 8);
+        ctx->donor_last_cols = cols;
+        ctx->donor_valid = true;
+    }
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->stats_last_n = sn;
     ctx->stats_n = 0;
@@ -1553,6 +1680,10 @@ static int finish_scalars(vtx_ctx* ctx)
     if (band_overflow)
         return set_err(ctx, VTX_E_UNSUPPORTED, "band model: %llu alignments had more k-mer hits than the work buffers hold (reads x windows too large); "
                                                "they were scored with the full matrix", (unsigned long long)band_overflow);
+    if (donor_bad)
+        return set_err(ctx, VTX_E_INVALID, "%llu loci have a row outside the donor dosage table given to vtx_set_donors (%llu rows); "
+                                           "they were left out of the donor log-likelihoods", (unsigned long long)donor_bad,
+                       (unsigned long long)ctx->donor_rows);
     if (violated)
         return set_err(ctx, VTX_E_INVALID, "%llu loci of a device batch exceeded the bounds given to vtx_submit_device(_ex) (longest read / widest "
                                            "haplotype window); they were skipped, the result is incomplete", (unsigned long long)violated);

@@ -590,6 +590,28 @@ class Engine:
         raw = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint32)), shape=(int(n.value) * len(_capi.LOCUS_STATS_FIELDS),))
         return raw.copy().view(self.LOCUS_STATS_DTYPE)
 
+    def set_donors(self, dosage: np.ndarray, error_rate: float = 0.01):
+        """Donor genotypes for per-cell demultiplexing (vtx_set_donors, include/vartrix_b200.h): dosage is uint8[rows, D], the
+        ALT dosage 0..2 of donor d at matrix row `row`, or _capi.GT_MISSING; 2 <= D <= 32, 1e-6 <= error_rate <= 0.25.  Before
+        the first submit."""
+        g = np.ascontiguousarray(dosage, dtype=np.uint8)
+        if g.ndim != 2:
+            raise ValueError(f"dosage must be a [rows, donors] array, not shape {g.shape}")
+        self._ck(self._L.vtx_set_donors(self._h, g.shape[1], g.shape[0], g.ctypes.data if g.size else None, float(error_rate)),
+                 "vtx_set_donors")
+
+    def donor_ll(self):
+        """-> (ll int64[cols, H] x 2^24 in vtx_set_donors' hypothesis order, counts uint64[cols, 3] = variants, ref, alt),
+        summed over the submits before the last finish (vtx_donor_ll_get)."""
+        ll, cnt = C.POINTER(C.c_int64)(), C.POINTER(C.c_uint64)()
+        n_cols, n_hyp = C.c_uint32(), C.c_uint32()
+        self._ck(self._L.vtx_donor_ll_get(self._h, C.byref(ll), C.byref(cnt), C.byref(n_cols), C.byref(n_hyp)), "vtx_donor_ll_get")
+        nc, nh = int(n_cols.value), int(n_hyp.value)
+        if nc == 0:
+            return np.zeros((0, nh), np.int64), np.zeros((0, 3), np.uint64)
+        return (np.ctypeslib.as_array(ll, shape=(nc * nh,)).reshape(nc, nh).copy(),
+                np.ctypeslib.as_array(cnt, shape=(nc * 3,)).reshape(nc, 3).copy())
+
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()
 
