@@ -19,7 +19,7 @@ $(LIB): $(CSRC)/vtx_api.cu $(wildcard $(CSRC)/*.cuh) include/vartrix_b200.h
 	@grep -E "error|warning" $(LIBDIR)/ptxas.log | grep -v "ptxas info" || true
 
 # C++ host: BAM/VCF/FASTA decode + staging + CLI with the vartrix flag surface, on top of the C ABI
-$(CLI): $(HOSTSRC)/main.cpp $(HOSTSRC)/stager.hpp $(HOSTSRC)/inputs.hpp $(HOSTSRC)/bam_reader.hpp $(HOSTSRC)/inflate_fast.hpp $(HOSTSRC)/crc32_fast.hpp $(CSRC)/vtx_base_quality.cuh $(CSRC)/vtx_donors.cuh include/vartrix_b200.h $(LIB)
+$(CLI): $(HOSTSRC)/main.cpp $(HOSTSRC)/stager.hpp $(HOSTSRC)/inputs.hpp $(HOSTSRC)/bam_reader.hpp $(HOSTSRC)/inflate_fast.hpp $(HOSTSRC)/crc32_fast.hpp $(CSRC)/vtx_record.cuh $(CSRC)/vtx_donors.cuh include/vartrix_b200.h $(LIB)
 	@mkdir -p vartrix_b200/bin
 	g++ -O2 -std=c++17 -Wall -Wextra -o $@.tmp $(HOSTSRC)/main.cpp -L$(LIBDIR) -lvartrix_b200 -lz -lpthread -Wl,-rpath,'$$ORIGIN/../lib'
 	@mv -f $@.tmp $@

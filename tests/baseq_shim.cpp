@@ -1,4 +1,4 @@
-// test shim: the --min-base-quality decision body (vtx::stage::base_quality_ok, vartrix_b200/csrc/vtx_base_quality.cuh),
+// test shim: the --min-base-quality decision body (vtx::stage::base_quality_ok, vartrix_b200/csrc/vtx_record.cuh),
 // reached through vtx_stage.cuh as locus_cands reaches it on the device, run serially on the CPU over (record, locus) pairs.
 #include "../vartrix_b200/csrc/vtx_stage.cuh"
 

@@ -55,3 +55,16 @@ extern "C" int vtx_test_stage_dev(const uint8_t* stream, uint64_t stream_len, in
     out->metrics[3] = met.num_duplicates; out->metrics[4] = met.num_not_useful;
     return 0;
 }
+
+// the shared useful_alignment (vartrix_b200/csrc/vtx_record.cuh) on a minimal record at `pos`: the 32-byte header, a 1-byte
+// name and the CIGAR, as the oracle's vtxo_useful_alignment takes them
+extern "C" int vtx_test_useful_alignment(int64_t pos, const uint32_t* cigar, int32_t n_cigar, int64_t start, int64_t end)
+{
+    std::vector<uint8_t> b(33 + 4 * size_t(n_cigar), 0);
+    const uint32_t p = uint32_t(int32_t(pos)), nc = uint32_t(n_cigar);
+    memcpy(&b[4], &p, 4);                // little-endian host, as the BAM layout
+    b[8] = 1;                            // l_read_name: the NUL
+    b[12] = uint8_t(nc); b[13] = uint8_t(nc >> 8);
+    if (n_cigar) memcpy(&b[33], cigar, 4 * size_t(n_cigar));
+    return vtx::stage::useful_alignment(b.data(), start, end) ? 1 : 0;
+}

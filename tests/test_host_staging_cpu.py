@@ -326,6 +326,31 @@ def stage_dev(tmp_path_factory):
     return ctypes.CDLL(so)
 
 
+def test_shared_useful_alignment_equals_oracle_case_by_case(oracle, stage_dev):
+    """Both stagers call one useful_alignment (csrc/vtx_record.cuh), so the host-versus-device comparisons cannot tell it
+    from the reference.  The oracle's vtxo_useful_alignment can: the CIGAR table of test_oracle_cpu's
+    test_useful_alignment_cigar_rules, plus an interior H (after an M, and in the leading section after a P), a leading N and
+    an =/X block, at every locus near the read."""
+    import ctypes
+    code = {"M": 0, "I": 1, "D": 2, "N": 3, "S": 4, "H": 5, "P": 6, "=": 7, "X": 8}
+    ua = oracle.lib().vtxo_useful_alignment
+    mine = stage_dev.vtx_test_useful_alignment
+    mine.restype = ctypes.c_int
+    mine.argtypes = [ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_int64]
+    cigars = [[(50, "M")], [(10, "M"), (100, "N"), (10, "M")], [(10, "M"), (5, "D"), (10, "M")], [(5, "S"), (10, "M")],
+              [(5, "D"), (10, "M")],
+              [(10, "M"), (5, "H"), (10, "M")], [(2, "P"), (5, "H"), (10, "M")], [(5, "N"), (10, "M")], [(10, "="), (2, "X"), (10, "=")]]
+    n_true = 0
+    for ops in cigars:
+        a = np.array([(n << 4) | code[o] for n, o in ops], np.uint32)
+        for start in range(90, 240):
+            for end in (start + 1, start + 3):
+                want = ua(100, a.ctypes.data, len(a), start, end)
+                assert mine(100, a.ctypes.data, len(a), start, end) == want, (ops, start, end)
+                n_true += want
+    assert n_true > 0
+
+
 def _run_stage_dev(lib, stream, d, mapq, primary, nodup, umi, tag):
     import ctypes
 

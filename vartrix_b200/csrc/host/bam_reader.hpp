@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "../../../include/vartrix_b200.h"
+#include "../vtx_record.cuh"
 #include "crc32_fast.hpp"
 #include "inflate_fast.hpp"
 
@@ -350,53 +351,15 @@ struct BamRecord {
     const uint8_t* seq() const { return cigar() + 4 * n_cigar(); }
     const uint8_t* aux() const { return seq() + (l_seq() + 1) / 2 + l_seq(); }
     const uint8_t* end() const { return p + len; }
-    // htslib bam_endpos: pos + reference length of the CIGAR; pos + 1 when unmapped / no CIGAR / zero length
+    // htslib bam_endpos (vtx::stage::ref_end): pos + reference length of the CIGAR; pos + 1 when unmapped / zero length
     int64_t endpos() const { return endpos_of(p); }
-    static int64_t endpos_of(const uint8_t* d)      // d = the record without its block_size prefix
-    {
-        int64_t rlen = 0;
-        if (!(rd16(d + 14) & 4)) {
-            const uint8_t* c = d + 32 + d[8];
-            const uint32_t nc = rd16(d + 12);
-            for (uint32_t i = 0; i < nc; ++i) {
-                const uint32_t v = rd32(c + 4 * i), op = v & 0xF;
-                if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rlen += v >> 4;
-            }
-        }
-        return int64_t(int32_t(rd32(d + 4))) + (rlen > 0 ? rlen : 1);
-    }
-    // first aux field named `tag`: value bytes when its type is 'Z' (Record::aux -> Aux::String), else nullptr
+    static int64_t endpos_of(const uint8_t* d) { return vtx::stage::ref_end(d); }      // d = the record without its block_size prefix
+    // first aux field named `tag`: value bytes when its type is 'Z' (vtx::stage::aux_z), else nullptr
     const uint8_t* aux_z(const char tag[2], uint32_t* len) const
     {
-        const uint8_t* p = aux(); const uint8_t* e = end();
-        while (p + 3 <= e) {
-            const bool hit = p[0] == uint8_t(tag[0]) && p[1] == uint8_t(tag[1]);
-            const uint8_t ty = p[2];
-            p += 3;
-            if (ty == 'Z' || ty == 'H') {
-                const uint8_t* q = static_cast<const uint8_t*>(memchr(p, 0, size_t(e - p)));
-                if (!q) return nullptr;
-                if (hit) { if (ty == 'Z') { *len = uint32_t(q - p); return p; } return nullptr; }
-                p = q + 1;
-            } else {
-                size_t sz;
-                switch (ty) {
-                case 'A': case 'c': case 'C': sz = 1; break;
-                case 's': case 'S': sz = 2; break;
-                case 'i': case 'I': case 'f': sz = 4; break;
-                case 'B': {
-                    if (p + 5 > e) return nullptr;
-                    const uint8_t sub = p[0]; const uint32_t cnt = rd32(p + 1);
-                    const size_t es = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : 4;
-                    sz = 5 + size_t(cnt) * es; break;
-                }
-                default: return nullptr;
-                }
-                if (hit) return nullptr;
-                p += sz;
-            }
-        }
-        return nullptr;
+        const uint8_t* a = aux();
+        uint32_t off = 0;
+        return vtx::stage::aux_z(a, end(), uint8_t(tag[0]), uint8_t(tag[1]), &off, len) ? a + off : nullptr;
     }
 };
 

@@ -334,7 +334,7 @@ void stage_into_arena(const StagedShard& s, Arena& a, vtx_batch2* b)
 // vtx_locus_stats is 22 u32 counters in declaration order: the writer handles an entry as that array (a copy, not a cast)
 constexpr int kStatsWords = 22;
 static_assert(sizeof(vtx_locus_stats) == kStatsWords * sizeof(uint32_t), "vtx_locus_stats: 22 counters, no padding");
-static_assert(offsetof(vtx_locus_stats, fetched) == 1 * 4 && offsetof(vtx_locus_stats, low_base_quality) == 6 * 4 &&
+static_assert(offsetof(vtx_locus_stats, fetched) == 1 * 4 && offsetof(vtx_locus_stats, low_base_quality) == (1 + vtx::stage::kLowBaseQuality) * 4 &&
               offsetof(vtx_locus_stats, scored) == 9 * 4 && offsetof(vtx_locus_stats, cells_multi_unknown) == 21 * 4,
               "vtx_locus_stats field order");
 using StatsWords = std::array<uint32_t, kStatsWords>;      // [0] row, [1..6] fetched .. low_base_quality, [7..21] the rest
@@ -350,7 +350,8 @@ bool write_variant_stats(const std::string& path, const std::vector<VcfRecord>& 
         submitted[e.row] = 1;
     }
     for (size_t i = 0; i < host_rows.size(); ++i)
-        for (int k = 0; k < 6; ++k) row[host_rows[i]][1 + k] += host_filters[i * 6 + k];     // the stager's fetched .. low_base_quality
+        for (int k = 0; k < vtx::stage::kNumCounters; ++k)      // the stager's record counters, in the columns fetched .. low_base_quality
+            row[host_rows[i]][1 + k] += host_filters[i * vtx::stage::kNumCounters + k];
     FILE* f = fopen(path.c_str(), "wb");
     if (!f) return false;
     fputs("variant\tchrom\tpos\tref\talt\tstatus\tfetched\tlow_mapq\tnon_primary\tduplicate\tnot_useful\tlow_base_quality\t"
@@ -563,7 +564,7 @@ int main(int argc, char** argv)
     }
 
     StageArgs sa;
-    sa.padding = o.padding; sa.mapq = uint32_t(o.mapq); sa.primary_only = o.primary; sa.no_duplicates = o.no_dups;
+    sa.padding = o.padding; sa.mapq_min = uint32_t(o.mapq); sa.primary_only = o.primary; sa.no_duplicates = o.no_dups;
     sa.bam_tag[0] = o.bam_tag[0]; sa.bam_tag[1] = o.bam_tag[1];
     sa.with_umi = o.umi || o.collapse_mates || dumping;      // without --umi the engine never looks at the UB keys: they are not staged
     sa.name_keys = o.collapse_mates;

@@ -10,7 +10,7 @@
 #include <vector>
 
 #include "../../../include/vartrix_b200.h"
-#include "../vtx_base_quality.cuh"
+#include "../vtx_record.cuh"
 #include "bam_reader.hpp"
 #include "inputs.hpp"
 
@@ -26,49 +26,27 @@ struct HostMetrics {             // the host-side share of main.rs:449-459
         num_duplicates += o.num_duplicates; num_not_useful += o.num_not_useful; num_invalid_recs += o.num_invalid_recs;
         num_multiallelic_recs += o.num_multiallelic_recs; num_low_base_quality += o.num_low_base_quality;
     }
+    void add(const uint32_t (&c)[vtx::stage::kNumCounters])       // one locus's record counters
+    {
+        using namespace vtx::stage;
+        num_reads += c[kFetched]; num_low_mapq += c[kLowMapq]; num_non_primary += c[kNonPrimary];
+        num_duplicates += c[kDuplicate]; num_not_useful += c[kNotUseful]; num_low_base_quality += c[kLowBaseQuality];
+    }
 };
 
-struct StageArgs {
+struct StageArgs : vtx::stage::RecordFilters {     // --mapq, --primary-alignments, --no-duplicates, --min-base-quality
     int64_t padding = 100;       // --padding
-    uint32_t mapq = 0;           // --mapq
-    bool primary_only = false;   // --primary-alignments
-    bool no_duplicates = false;  // --no-duplicates
     char bam_tag[2] = { 'C', 'B' };
     bool valid[256] = {};        // --valid-chars
     bool with_umi = true;        // stage the UB keys (--umi, or a dump for the tests); without --umi nobody reads them
     bool name_keys = false;      // --collapse-mates: the staged key is the QNAME (per-shard interner), not the UB tag
-    uint32_t min_base_quality = 0;   // --min-base-quality (0: off)
     bool locus_filters = false;  // --out-variant-stats: keep the record-filter counters per locus (StagedShard::locus_filters)
     // --gpu-inflate: the BGZF members of a shard's loci are inflated in one device call (vtx_bgzf_inflate) instead of one
     // by one on the staging thread; empty = host inflate
     Bgzf::BulkInflate bulk_inflate;
 };
 
-// vtx_pack_cb (include/vartrix_b200.h), kept local so that staging can run without the CUDA library: an injective code of
-// [ACGT]{1,24}(-N)?, N = 1..99 without a leading zero; VTX_NO_CB_KEY for anything else (the tag is then staged as bytes)
-inline uint64_t pack_cb(const uint8_t* s, uint32_t len)
-{
-    uint32_t n = 0;
-    uint64_t k = 0;
-    while (n < len && n < 25) {
-        uint64_t c;
-        const uint8_t b = s[n];
-        if (b == 'A') c = 0; else if (b == 'C') c = 1; else if (b == 'G') c = 2; else if (b == 'T') c = 3; else break;
-        if (n == 24) return VTX_NO_CB_KEY;
-        k = (k << 2) | c;
-        ++n;
-    }
-    if (n == 0) return VTX_NO_CB_KEY;
-    uint64_t suffix = 0;
-    if (n < len) {
-        if (s[n] != '-') return VTX_NO_CB_KEY;
-        const uint32_t d = len - n - 1;
-        if (d < 1 || d > 2 || s[n + 1] < '1' || s[n + 1] > '9') return VTX_NO_CB_KEY;
-        suffix = uint64_t(s[n + 1] - '0');
-        if (d == 2) { if (s[n + 2] < '0' || s[n + 2] > '9') return VTX_NO_CB_KEY; suffix = suffix * 10 + uint64_t(s[n + 2] - '0'); }
-    }
-    return (k << 12) | (uint64_t(n) << 7) | suffix;
-}
+// the tag bytes of a vtx::stage::pack_cb code
 inline std::string unpack_cb(uint64_t key)
 {
     const uint32_t n = uint32_t(key >> 7) & 31u, suffix = uint32_t(key & 127u);
@@ -89,8 +67,8 @@ struct StagedShard {
     bool identity = true;        // candidate c is read c so far (no read shared between loci)
     bool with_umi = true;        // read_umi_key is filled
     HostMetrics met;
-    // per staged locus: fetched, low mapq, non-primary, duplicate, not useful, low base quality (--out-variant-stats; the
-    // device counts the rest of vtx_locus_stats)
+    // per staged locus: the vtx::stage::kNumCounters record counters (--out-variant-stats; the device counts the rest of
+    // vtx_locus_stats)
     std::vector<uint32_t> locus_filters;
 
     void clear()          // keeps the capacity: shards are recycled so steady-state staging does not page-fault
@@ -124,23 +102,11 @@ class UmiInterner {
 public:
     uint64_t key(const uint8_t* s, uint32_t len)
     {
-        const uint64_t k = pack(s, len);
+        const uint64_t k = vtx::stage::pack_umi(s, len);
         if (k != VTX_NO_UMI) return k;
         std::lock_guard<std::mutex> g(mu_);
         auto it = map_.emplace(std::string(reinterpret_cast<const char*>(s), len), map_.size()).first;
         return (1ull << 61) | it->second;
-    }
-    // same encoding as vtx_pack_umi (kept local so that staging can run without the CUDA library)
-    static uint64_t pack(const uint8_t* s, uint32_t len)
-    {
-        if (len > 18) return VTX_NO_UMI;
-        uint64_t k = 0;
-        for (uint32_t i = 0; i < len; ++i) {
-            uint64_t c;
-            switch (s[i]) { case 'A': c = 0; break; case 'C': c = 1; break; case 'G': c = 2; break; case 'T': c = 3; break; case 'N': c = 4; break; default: return VTX_NO_UMI; }
-            k = (k << 3) | c;
-        }
-        return (k << 5) | len;
     }
 private:
     std::mutex mu_;
@@ -163,36 +129,6 @@ private:
     std::unordered_map<std::string, uint64_t> map_;
     uint64_t next_ = 0;
 };
-
-// rust-htslib 0.36 CigarStringView::read_pos(p, include_softclips = false, include_dels = true) folded
-// into useful_alignment (main.rs:790-806): is there a p in start..=end with an aligned base or a deletion?
-inline bool useful_alignment(const BamRecord& rec, int64_t start, int64_t end)
-{
-    const uint8_t* cg = rec.cigar();
-    const uint32_t nc = rec.n_cigar();
-    auto op_at = [&](uint32_t i) { return rd32(cg + 4 * i) & 0xF; };
-    auto len_at = [&](uint32_t i) { return int64_t(rd32(cg + 4 * i) >> 4); };
-    // leading section: first of M,=,X,I,S starts the walk; leading D/N or an interior H is an error (read skipped)
-    uint32_t i0 = 0;
-    while (i0 < nc) {
-        const uint32_t op = op_at(i0);
-        if (op == 0 || op == 7 || op == 8 || op == 1 || op == 4) break;
-        if (op == 2 || op == 3) return false;
-        if (op == 5 && i0 != 0 && i0 != nc - 1) return false;
-        ++i0;
-    }
-    if (i0 >= nc) return false;
-    for (int64_t p = start; p <= end; ++p) {          // inclusive end, main.rs:794
-        int64_t rpos = rec.pos();
-        for (uint32_t i = i0; i < nc && rpos <= p; ++i) {
-            const uint32_t op = op_at(i); const int64_t len = len_at(i);
-            if (op == 0 || op == 7 || op == 8 || op == 2) { if (p >= rpos && p < rpos + len) return true; rpos += len; }
-            else if (op == 3) rpos += len;
-            else if (op == 5) { if (i != nc - 1) return false; break; }
-        }
-    }
-    return false;
-}
 
 inline void pad16(std::vector<uint8_t>& v) { while (v.size() & 15) v.push_back(0); }
 
@@ -235,6 +171,37 @@ private:
     size_t n_ = 0;
 };
 
+enum class Window { kScored, kMultiallelic, kInvalidAlt, kFastaError };
+
+// VCF record `row` at the locus [start, end) -> its haplotype windows (construct_haplotypes, main.rs:619-684, 958-994).  One
+// read of the reference window; its two flanks are the alt haplotype's flanks (same FASTA bytes).  A scored record appends its
+// row and both windows to the shard (StagedShard or DeviceShard); a multi-allelic or invalid-ALT one is counted in its metrics.
+template <class Shard>
+inline Window stage_windows(const VcfRecord& v, uint32_t row, int64_t start, int64_t end, const Fasta& fa, const StageArgs& a,
+                            Shard* out, std::string* err)
+{
+    if (v.alleles.size() > 2) { out->met.num_multiallelic_recs++; return Window::kMultiallelic; }        // main.rs:646-653
+    const int64_t L = fa.length(v.chrom);
+    if (L < 0) { *err = "Requested chromosome " + v.chrom + " was not found in fasta"; return Window::kFastaError; }
+    static thread_local std::string ref_hap, alt_hap;
+    const int64_t w0 = std::max<int64_t>(start - a.padding, 0), w1 = std::min(end + a.padding, L);
+    if (end > L || !fa.fetch_upper(v.chrom, w0, w1, &ref_hap)) {
+        *err = "FASTA fetch failed at " + v.chrom + ":" + std::to_string(v.pos0);
+        return Window::kFastaError;
+    }
+    alt_hap.assign(ref_hap, 0, size_t(start - w0));                    // FASTA[max(start - pad, 0), start)
+    if (v.alleles.size() == 2) alt_hap += v.alleles[1];                 // main.rs:656-659: no ALT allele is an empty one
+    alt_hap.append(ref_hap, size_t(end - w0), std::string::npos);       // FASTA[end, min(end + pad, L))
+    for (unsigned char c : alt_hap)
+        if (!a.valid[c]) { out->met.num_invalid_recs++; return Window::kInvalidAlt; }                  // main.rs:675-684
+    out->locus_row.push_back(row);
+    pad16(out->hap_bytes); out->ref_off.push_back(uint32_t(out->hap_bytes.size())); out->ref_len.push_back(uint32_t(ref_hap.size()));
+    out->hap_bytes.insert(out->hap_bytes.end(), ref_hap.begin(), ref_hap.end());
+    pad16(out->hap_bytes); out->alt_off.push_back(uint32_t(out->hap_bytes.size())); out->alt_len.push_back(uint32_t(alt_hap.size()));
+    out->hap_bytes.insert(out->hap_bytes.end(), alt_hap.begin(), alt_hap.end());
+    return Window::kScored;
+}
+
 // What the host keeps doing when the device stages the reads itself (vtx_submit_bam): windows from the FASTA, the compressed
 // byte range of the loci's index chunks, the BGZF member table, the record boundaries the index knows.
 struct DeviceShard {
@@ -253,7 +220,7 @@ struct DeviceShard {
         b->ref_off = ref_off.data(); b->ref_len = ref_len.data(); b->alt_off = alt_off.data(); b->alt_len = alt_len.data();
         b->tid = tid; b->n_members = uint32_t(members.size()); b->members = members.data(); b->comp = comp.data(); b->comp_len = comp.empty() ? 0 : comp.size() - 16;
         b->n_entry = uint32_t(entry_off.size()); b->entry_off = entry_off.data();
-        b->mapq = a.mapq; b->primary_only = a.primary_only; b->no_duplicates = a.no_duplicates; b->bam_tag[0] = a.bam_tag[0]; b->bam_tag[1] = a.bam_tag[1];
+        b->mapq = a.mapq_min; b->primary_only = a.primary_only; b->no_duplicates = a.no_duplicates; b->bam_tag[0] = a.bam_tag[0]; b->bam_tag[1] = a.bam_tag[1];
     }
 };
 
@@ -268,28 +235,14 @@ inline bool stage_loci_device(const std::vector<VcfRecord>& recs, size_t lo, siz
     *out = DeviceShard();
     if (hi <= lo) return true;
     out->tid = bam.tid_of(recs[lo].chrom);
-    std::string ref_hap, alt_hap;
     std::vector<BaiChunk> chunks;
     for (size_t i = lo; i < hi; ++i) {
         const VcfRecord& v = recs[i];
         const int64_t start = v.pos0, end = v.pos0 + int64_t(v.alleles[0].size());      // main.rs:619-623
-        if (v.alleles.size() > 2) { out->met.num_multiallelic_recs++; continue; }       // main.rs:646-653
-        const std::string alt = v.alleles.size() == 2 ? v.alleles[1] : std::string();   // main.rs:656-659
-        const int64_t L = fa.length(v.chrom);
-        if (L < 0) { *err = "Requested chromosome " + v.chrom + " was not found in fasta"; return false; }
-        const int64_t w0 = std::max<int64_t>(start - a.padding, 0), w1 = std::min(end + a.padding, L);
-        if (end > L || !fa.fetch_upper(v.chrom, w0, w1, &ref_hap)) { *err = "FASTA fetch failed at " + v.chrom + ":" + std::to_string(v.pos0); return false; }
-        alt_hap.assign(ref_hap, 0, size_t(start - w0));
-        alt_hap += alt;
-        alt_hap.append(ref_hap, size_t(end - w0), std::string::npos);
-        bool ok = true;
-        for (unsigned char c : alt_hap) if (!a.valid[c]) { ok = false; break; }         // main.rs:675-684
-        if (!ok) { out->met.num_invalid_recs++; continue; }
-        out->locus_row.push_back(uint32_t(i)); out->locus_start.push_back(start); out->locus_end.push_back(end);
-        pad16(out->hap_bytes); out->ref_off.push_back(uint32_t(out->hap_bytes.size())); out->ref_len.push_back(uint32_t(ref_hap.size()));
-        out->hap_bytes.insert(out->hap_bytes.end(), ref_hap.begin(), ref_hap.end());
-        pad16(out->hap_bytes); out->alt_off.push_back(uint32_t(out->hap_bytes.size())); out->alt_len.push_back(uint32_t(alt_hap.size()));
-        out->hap_bytes.insert(out->hap_bytes.end(), alt_hap.begin(), alt_hap.end());
+        const Window w = stage_windows(v, uint32_t(i), start, end, fa, a, out, err);
+        if (w == Window::kFastaError) return false;
+        if (w != Window::kScored) continue;
+        out->locus_start.push_back(start); out->locus_end.push_back(end);
         bam.region_chunks(out->tid, start, end, &chunks);
     }
     pad16(out->hap_bytes);
@@ -354,47 +307,20 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
     static thread_local NameInterner names;                 // --collapse-mates: this shard's QNAME keys
     names.clear();
     BamRecord rec;
-    std::string ref_hap, alt_hap;
     out->cand_start.push_back(0);
     for (size_t i = lo; i < hi; ++i) {
         const VcfRecord& v = recs[i];
         const int64_t start = v.pos0, end = v.pos0 + int64_t(v.alleles[0].size());      // main.rs:619-623
-        if (v.alleles.size() > 2) { out->met.num_multiallelic_recs++; continue; }       // main.rs:646-653
-        const std::string alt = v.alleles.size() == 2 ? v.alleles[1] : std::string();   // main.rs:656-659
-        const int64_t L = fa.length(v.chrom);
-        if (L < 0) { *err = "Requested chromosome " + v.chrom + " was not found in fasta"; return false; }
-        // construct_haplotypes, main.rs:958-994
-        // one read of the reference window; its two flanks are the alt haplotype's flanks (same FASTA bytes)
-        const int64_t w0 = std::max<int64_t>(start - a.padding, 0), w1 = std::min(end + a.padding, L);
-        if (end > L || !fa.fetch_upper(v.chrom, w0, w1, &ref_hap)) {
-            *err = "FASTA fetch failed at " + v.chrom + ":" + std::to_string(v.pos0);
-            return false;
-        }
-        alt_hap.assign(ref_hap, 0, size_t(start - w0));            // FASTA[max(start - pad, 0), start)
-        alt_hap += alt;
-        alt_hap.append(ref_hap, size_t(end - w0), std::string::npos);   // FASTA[end, min(end + pad, L))
-        bool ok = true;
-        for (unsigned char c : alt_hap) if (!a.valid[c]) { ok = false; break; }         // main.rs:675-684
-        if (!ok) { out->met.num_invalid_recs++; continue; }
-        out->locus_row.push_back(uint32_t(i));
-        pad16(out->hap_bytes); out->ref_off.push_back(uint32_t(out->hap_bytes.size())); out->ref_len.push_back(uint32_t(ref_hap.size()));
-        out->hap_bytes.insert(out->hap_bytes.end(), ref_hap.begin(), ref_hap.end());
-        pad16(out->hap_bytes); out->alt_off.push_back(uint32_t(out->hap_bytes.size())); out->alt_len.push_back(uint32_t(alt_hap.size()));
-        out->hap_bytes.insert(out->hap_bytes.end(), alt_hap.begin(), alt_hap.end());
+        const Window w = stage_windows(v, uint32_t(i), start, end, fa, a, out, err);
+        if (w == Window::kFastaError) return false;
+        if (w != Window::kScored) continue;
 
-        const HostMetrics m0 = out->met;
+        uint32_t c[vtx::stage::kNumCounters] = {};
         const int tid = bam.tid_of(v.chrom);
         if (tid >= 0 && bam.fetch(tid, start, end)) {                                    // main.rs:822-826
             while (bam.next(&rec)) {
-                out->met.num_reads++;
-                const uint32_t fl = rec.flag();
-                if (rec.mapq() < a.mapq) { out->met.num_low_mapq++; continue; }                               // 833
-                if (a.primary_only && (fl & 0x100 || fl & 0x800)) { out->met.num_non_primary++; continue; }   // 841
-                if (a.no_duplicates && (fl & 0x400)) { out->met.num_duplicates++; continue; }                 // 849
-                if (!useful_alignment(rec, start, end)) { out->met.num_not_useful++; continue; }              // 857
-                if (a.min_base_quality && !vtx::stage::base_quality_ok(rec.p, start, end, a.min_base_quality)) {
-                    out->met.num_low_base_quality++; continue;
-                }
+                ++c[vtx::stage::kFetched];                                               // 831
+                if (const int drop = vtx::stage::drop_reason(rec.flag(), rec.mapq(), rec.p, start, end, a)) { ++c[drop]; continue; }
                 bool fresh = false;
                 const uint32_t rid = read_index.find_or_insert(rec.voff, uint32_t(out->read_len.size()), &fresh);
                 if (fresh) {
@@ -407,7 +333,7 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
                     const uint8_t* cb = rec.aux_z(a.bam_tag, &n);                                             // main.rs:737-750
                     uint64_t key = VTX_NO_CB_KEY;
                     if (cb && n <= 0xFFFF) {
-                        key = pack_cb(cb, n);
+                        key = vtx::stage::pack_cb(cb, n);
                         if (key == VTX_NO_CB_KEY) {        // a tag the code cannot express travels as bytes
                             key = VTX_CB_EXOTIC | uint64_t(out->cb_off.size() - 1);
                             out->cb_bytes.insert(out->cb_bytes.end(), cb, cb + n);
@@ -429,12 +355,8 @@ inline bool stage_loci(const std::vector<VcfRecord>& recs, size_t lo, size_t hi,
             if (bam.bad()) { *err = bam.error(); return false; }            // corrupt / truncated BAM: abort (main.rs:830)
         }
         out->cand_start.push_back(out->cand_read.size());
-        const HostMetrics& m1 = out->met;
-        if (a.locus_filters)
-            for (uint64_t d : { m1.num_reads - m0.num_reads, m1.num_low_mapq - m0.num_low_mapq, m1.num_non_primary - m0.num_non_primary,
-                                m1.num_duplicates - m0.num_duplicates, m1.num_not_useful - m0.num_not_useful,
-                                m1.num_low_base_quality - m0.num_low_base_quality })
-                out->locus_filters.push_back(uint32_t(d));
+        out->met.add(c);
+        if (a.locus_filters) out->locus_filters.insert(out->locus_filters.end(), c, c + vtx::stage::kNumCounters);
     }
     while (out->read_nib.size() & 3) out->read_nib.push_back(0);
     pad16(out->hap_bytes);

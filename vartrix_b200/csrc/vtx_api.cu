@@ -337,7 +337,7 @@ struct DevBatch {   // device pointers
     uint32_t class_mask = ~0u;       // tile classes that may get tiles (host batches: from the windows; device batches: all)
     uint32_t max_read_len = 0, max_hap_len = 0;
     uint64_t max_depth = ~0ull;      // most candidates of one locus (unknown for device batches: assume deep)
-    const uint32_t* lfilt = nullptr; // [n_loci][6] record-filter counters of a vtx_submit_bam shard (vtx_set_locus_stats)
+    const uint32_t* lfilt = nullptr; // [n_loci][stage::kNumCounters] record-filter counters of a vtx_submit_bam shard (vtx_set_locus_stats)
 };
 
 // the allow_* switches of run_sw, shared with the host-side class mask
@@ -1257,7 +1257,7 @@ int vtx_set_barcodes(vtx_ctx* ctx, const uint8_t* bytes, const uint32_t* off, ui
     std::vector<uint64_t> kkey(cap, kNoCbKey);
     std::vector<uint32_t> kidx(cap, 0);
     for (uint32_t i = 0; i < n; ++i) {
-        const uint64_t k = pack_cb(bytes + off[i], off[i + 1] - off[i]);
+        const uint64_t k = stage::pack_cb(bytes + off[i], off[i + 1] - off[i]);
         if (k == kNoCbKey) continue;
         uint32_t h = uint32_t(mix64(k)) & (cap - 1);
         while (kkey[h] != kNoCbKey) h = (h + 1) & (cap - 1);       // codes are injective and the strings distinct: no equal key
@@ -1411,10 +1411,11 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
     CK(cudaMemsetAsync(sl.scalars.p, 0, 256, ss));
     if (nm && (rc = launch_inflate(ctx, ss, sl.desc.p, nm, sl.comp.p, sl.stream.p, sl.status.p, d_sc, 1))) return fail_out(rc);
     stage::Params sp{};
-    sp.s = P<uint8_t>(sl.stream); sp.s_len = stream_len; sp.tid = sh->tid; sp.mapq_min = sh->mapq; sp.primary_only = sh->primary_only;
-    const bool name_keys = (ctx->cfg.flags & VTX_F_NAME_KEYS) != 0;       // the keys come from vtx_k_name_key, not from UB tags
-    sp.no_duplicates = sh->no_duplicates; sp.want_umi = ctx->cfg.use_umi && !name_keys ? 1 : 0; sp.tag0 = uint8_t(sh->bam_tag[0]); sp.tag1 = uint8_t(sh->bam_tag[1]);
+    sp.s = P<uint8_t>(sl.stream); sp.s_len = stream_len; sp.tid = sh->tid;
+    sp.mapq_min = sh->mapq; sp.primary_only = sh->primary_only != 0; sp.no_duplicates = sh->no_duplicates != 0;
     sp.min_base_quality = ctx->min_base_quality;
+    const bool name_keys = (ctx->cfg.flags & VTX_F_NAME_KEYS) != 0;       // the keys come from vtx_k_name_key, not from UB tags
+    sp.want_umi = ctx->cfg.use_umi && !name_keys ? 1 : 0; sp.tag0 = uint8_t(sh->bam_tag[0]); sp.tag1 = uint8_t(sh->bam_tag[1]);
     // ---- record boundaries ----
     const uint32_t n_seg = ne ? ne - 1 : 0;
     ENS(sl.seg_count, size_t(n_seg + 1) * 4); ENS(sl.seg_first, size_t(n_seg + 2) * 4);
@@ -1453,7 +1454,7 @@ int vtx_submit_bam(vtx_ctx* ctx, const vtx_bam_shard* sh)
         ENS(sl.status, std::max<size_t>(size_t(nm) * 4 + 16, sizeof(stage::LocusMetrics) + 16));
         stage::LocusMetrics* d_tmp = reinterpret_cast<stage::LocusMetrics*>(sl.status.p);
         CK(cudaMemsetAsync(d_tmp, 0, sizeof(stage::LocusMetrics), ss));
-        if (ctx->locus_stats) ENS(sl.lfilt, size_t(nl) * lstats::kFilters * 4);
+        if (ctx->locus_stats) ENS(sl.lfilt, size_t(nl) * stage::kNumCounters * 4);
         stage::vtx_k_locus_cands<<<blocks_for(nl, 64), 64, 0, ss>>>(sp, nl, P<int64_t>(sl.l_start), P<int64_t>(sl.l_end), n_rec, P<uint64_t>(sl.rec_off),
                                                                    P<int32_t>(sl.rec_tid), P<int32_t>(sl.rec_pos), P<int32_t>(sl.rec_end), P<uint32_t>(sl.rec_fm),
                                                                    d_sc + 2, d_sc + 3, 0, P<uint32_t>(sl.cand_count), nullptr, nullptr, nullptr, d_tmp,
@@ -1527,7 +1528,9 @@ int vtx_bam_metrics_get(vtx_ctx* ctx, vtx_bam_metrics* out)
     memset(out, 0, sizeof(*out));
     if (!ctx->stage_stream) return VTX_OK;
     CK(cudaSetDevice(ctx->device));
-    static_assert(sizeof(vtx_bam_metrics) == offsetof(stage::LocusMetrics, num_low_base_quality), "metric layouts must agree");
+    static_assert(sizeof(vtx_bam_metrics) == offsetof(stage::LocusMetrics, num_low_base_quality) &&
+                  offsetof(stage::LocusMetrics, num_low_base_quality) == stage::kLowBaseQuality * sizeof(unsigned long long),
+                  "metric layouts must agree");
     CK(cudaMemcpyAsync(out, ctx->bam_metrics.p, sizeof(*out), cudaMemcpyDeviceToHost, ctx->stage_stream));
     CK(cudaStreamSynchronize(ctx->stage_stream));
     return VTX_OK;
@@ -1616,7 +1619,7 @@ int vtx_donor_ll_get(vtx_ctx* ctx, const int64_t** ll, const uint64_t** counts, 
     return VTX_OK;
 }
 
-uint64_t vtx_pack_cb(const uint8_t* s, uint32_t len) { return (s || len == 0) ? pack_cb(s, len) : VTX_NO_CB_KEY; }
+uint64_t vtx_pack_cb(const uint8_t* s, uint32_t len) { return (s || len == 0) ? stage::pack_cb(s, len) : VTX_NO_CB_KEY; }
 
 int vtx_sync(vtx_ctx* ctx)
 {
@@ -1849,17 +1852,7 @@ int vtx_score_pairs(vtx_ctx* ctx, const vtx_batch* hb, uint64_t n_pairs, const u
     return VTX_OK;
 }
 
-uint64_t vtx_pack_umi(const uint8_t* s, uint32_t len)
-{
-    if (len > 18) return VTX_NO_UMI;
-    uint64_t k = 0;
-    for (uint32_t i = 0; i < len; ++i) {
-        uint64_t c;
-        switch (s[i]) { case 'A': c = 0; break; case 'C': c = 1; break; case 'G': c = 2; break; case 'T': c = 3; break; case 'N': c = 4; break; default: return VTX_NO_UMI; }
-        k = (k << 3) | c;
-    }
-    return (k << 5) | len;      // < 2^59: bits 59..61 stay clear for caller-interned ids
-}
+uint64_t vtx_pack_umi(const uint8_t* s, uint32_t len) { return stage::pack_umi(s, len); }
 
 
 // -------------------------------------------------------------------------------------------------

@@ -16,6 +16,8 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "vtx_record.cuh"
+
 #if defined(__CUDACC__)
 #define VTX_LS_HD __host__ __device__
 #else
@@ -31,7 +33,7 @@ enum : int {
     kReadsRef, kReadsAlt, kReadsUnknown, kReadsNone, kCallsRef, kCallsAlt, kCallsUnknown,
     kCells, kCellsRefOnly, kCellsAltOnly, kCellsBoth, kCellsMultiUnknown, kFields
 };
-constexpr int kFilters = 6;             // kFetched .. kLowBaseQuality: what locus_cands stores per locus
+static_assert(kNoCellBarcode - kFetched == stage::kNumCounters, "kFetched .. kLowBaseQuality: locus_cands' record counters, in their order");
 // the summed counters
 enum : int { sNoCb = 0, sNoUmi, sReadsRef, sReadsAlt, sReadsUnk, sCallsRef, sCallsAlt, sCallsUnk, sCells, sRefOnly, sAltOnly, sBoth, sMultiUnk, kSums };
 
@@ -48,7 +50,7 @@ struct Inputs {
     const uint32_t* ccnt;           // [slot][4] calls of a cell slot (after the collapse with use_umi)
     const uint32_t* cslot_col;      // [slot] column or kNoCell
     const uint32_t* locus_row;      // [n_loci]
-    const uint32_t* filters;        // [n_loci][kFilters] from locus_cands, nullptr: host batch
+    const uint32_t* filters;        // [n_loci][stage::kNumCounters] from locus_cands, nullptr: host batch
 };
 
 VTX_LS_HD inline void add_candidate(const Inputs& in, uint64_t c, uint32_t* s)
@@ -76,7 +78,7 @@ VTX_LS_HD inline void add_slot(const Inputs& in, uint32_t q, uint32_t* s)
 VTX_LS_HD inline void write_entry(const Inputs& in, uint32_t l, const uint32_t* s, uint32_t* out)
 {
     out[kRow] = in.locus_row[l];
-    for (int f = 0; f < kFilters; ++f) out[kFetched + f] = in.filters ? in.filters[size_t(l) * kFilters + f] : 0u;
+    for (int f = 0; f < stage::kNumCounters; ++f) out[kFetched + f] = in.filters ? in.filters[size_t(l) * stage::kNumCounters + f] : 0u;
     out[kNoCellBarcode] = s[sNoCb]; out[kNoUmi] = s[sNoUmi];
     const uint32_t scored = in.pair_start ? in.pair_start[l + 1] - in.pair_start[l] : 0u;
     out[kScored] = scored;

@@ -16,6 +16,7 @@
 #include "vtx_sw.cuh"
 #include "vtx_sw_split.cuh"
 #include "vtx_sw_fold.cuh"
+#include "vtx_record.cuh"
 
 namespace vtx {
 
@@ -66,33 +67,8 @@ __global__ void vtx_k_cb_lookup(BarcodeTable t, uint32_t n_reads, const uint8_t*
 }
 
 // ---- slim layout (vtx_batch2): cell tags travel as one injective u64 code per read -------------------------------
-constexpr uint64_t kNoCbKey = 0xFFFFFFFFFFFFFFFFull;
+using stage::kNoCbKey;                          // what stage::pack_cb returns for a tag it cannot code
 constexpr uint64_t kCbExotic = 0x8000000000000000ull;
-
-// [ACGT]{1,24}(-N)?, N = 1..99 without a leading zero -> bases (2 bits each) << 12 | n_bases << 7 | N ; else kNoCbKey
-__host__ __device__ inline uint64_t pack_cb(const uint8_t* s, uint32_t len)
-{
-    uint32_t n = 0;
-    uint64_t k = 0;
-    while (n < len && n < 25) {
-        uint64_t c;
-        const uint8_t b = s[n];
-        if (b == 'A') c = 0; else if (b == 'C') c = 1; else if (b == 'G') c = 2; else if (b == 'T') c = 3; else break;
-        if (n == 24) return kNoCbKey;
-        k = (k << 2) | c;
-        ++n;
-    }
-    if (n == 0) return kNoCbKey;
-    uint64_t suffix = 0;
-    if (n < len) {
-        if (s[n] != '-') return kNoCbKey;
-        const uint32_t d = len - n - 1;
-        if (d < 1 || d > 2 || s[n + 1] < '1' || s[n + 1] > '9') return kNoCbKey;
-        suffix = uint64_t(s[n + 1] - '0');
-        if (d == 2) { if (s[n + 2] < '0' || s[n + 2] > '9') return kNoCbKey; suffix = suffix * 10 + uint64_t(s[n + 2] - '0'); }
-    }
-    return (k << 12) | (uint64_t(n) << 7) | suffix;
-}
 
 __host__ __device__ inline uint64_t mix64(uint64_t x)
 {

@@ -5,7 +5,7 @@
 // threads and the reference does through rust-htslib (vartrix src/main.rs:822-865, 737-757, 790-806):
 //   fetch          every record of the contig with pos < end and bam_endpos > start, in file order   (main.rs:822-829)
 //   record filters mapq, --primary-alignments, --no-duplicates, useful_alignment, in that order      (main.rs:833-865)
-//                  then, with --min-base-quality, the judged bases' qualities (vtx_base_quality.cuh)
+//                  then the --min-base-quality floor: drop_reason (vtx_record.cuh), as on the host
 //   tags           CB (or --bam-tag) and UB: first aux field of that name, type Z                      (main.rs:737-757)
 //                  or, with --collapse-mates, the QNAME as the molecule key instead of UB (name_key below)
 // The record stream is walked from the BAI chunk starts that fall into the shard's range (record boundaries by
@@ -15,29 +15,23 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
-#include "vtx_base_quality.cuh"
+#include "vtx_record.cuh"
 
 namespace vtx {
 namespace stage {
 
 constexpr uint32_t kNoCb = 0xFFFFFFFFu;
-constexpr uint64_t kNoUmi = 0xFFFFFFFFFFFFFFFFull;
 
-struct Params {
+struct Params : RecordFilters {  // vtx_bam_shard's mapq / primary_only / no_duplicates, vtx_set_min_base_quality
     const uint8_t* s;            // inflated stream: the members' outputs back to back
     uint64_t s_len;
     int32_t tid;                 // contig of every locus of the shard
-    uint32_t mapq_min;
-    int32_t primary_only, no_duplicates, want_umi;
+    int32_t want_umi;
     uint8_t tag0, tag1;          // --bam-tag
-    uint32_t min_base_quality;   // --min-base-quality (0: off)
 };
 
 // error bits (first word of `err`): the shard is then re-staged on the host, which produces the message
 enum : uint32_t { kErrWalk = 1, kErrRecord = 2, kErrExoticUmi = 4, kErrLongRead = 8 };
-
-__host__ __device__ inline uint32_t ld32(const uint8_t* p) { return uint32_t(p[0]) | (uint32_t(p[1]) << 8) | (uint32_t(p[2]) << 16) | (uint32_t(p[3]) << 24); }
-__host__ __device__ inline uint32_t ld16(const uint8_t* p) { return uint32_t(p[0]) | (uint32_t(p[1]) << 8); }
 
 // The per-item bodies below are __host__ __device__: the kernels at the end of the file are one-line wrappers, and
 // tests/stage_dev_shim.cpp runs the same bodies serially on the CPU against the host stager (tests/test_host_staging_cpu.py).
@@ -109,16 +103,8 @@ __host__ __device__ inline void parse_record(const Params& P, uint32_t i, const 
 {
     const uint8_t* b = P.s + rec_off[i] + 4;
     const int32_t pos = int32_t(ld32(b + 4));
-    const uint32_t flag = ld16(b + 14), nc = ld16(b + 12);
-    int64_t rlen = 0;
-    if (!(flag & 4)) {
-        const uint8_t* c = b + 32 + b[8];
-        for (uint32_t q = 0; q < nc; ++q) {
-            const uint32_t v = ld32(c + 4 * q), op = v & 0xF;
-            if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rlen += v >> 4;
-        }
-    }
-    const int64_t e = int64_t(pos) + (rlen > 0 ? rlen : 1);
+    const uint32_t flag = ld16(b + 14);
+    const int64_t e = ref_end(b);
     const int32_t tid = int32_t(ld32(b));
     rec_tid[i] = tid;
     // a range of the shard's contig holds only its records; should the index ever hand out a tail of the next contig (or of
@@ -129,43 +115,17 @@ __host__ __device__ inline void parse_record(const Params& P, uint32_t i, const 
     if (tid == P.tid) take_max(max_span, uint32_t(e - pos > 0xFFFFFFFFll ? 0xFFFFFFFFu : uint32_t(e - pos)));
 }
 
-// rust-htslib 0.36 CigarStringView::read_pos(p, include_softclips = false, include_dels = true) folded into
-// useful_alignment (main.rs:790-806): is there a p in start..=end with an aligned base or a deletion?
-__host__ __device__ inline bool useful_alignment(const uint8_t* b, int64_t start, int64_t end)
-{
-    const uint8_t* cg = b + 32 + b[8];
-    const uint32_t nc = ld16(b + 12);
-    const int64_t pos0 = int32_t(ld32(b + 4));
-    uint32_t i0 = 0;
-    while (i0 < nc) {            // leading section: first of M,=,X,I,S starts the walk; leading D/N or an interior H is an error
-        const uint32_t op = ld32(cg + 4 * i0) & 0xF;
-        if (op == 0 || op == 7 || op == 8 || op == 1 || op == 4) break;
-        if (op == 2 || op == 3) return false;
-        if (op == 5 && i0 != 0 && i0 != nc - 1) return false;
-        ++i0;
-    }
-    if (i0 >= nc) return false;
-    for (int64_t p = start; p <= end; ++p) {          // inclusive end, main.rs:794
-        int64_t rpos = pos0;
-        for (uint32_t i = i0; i < nc && rpos <= p; ++i) {
-            const uint32_t v = ld32(cg + 4 * i), op = v & 0xF; const int64_t len = int64_t(v >> 4);
-            if (op == 0 || op == 7 || op == 8 || op == 2) { if (p >= rpos && p < rpos + len) return true; rpos += len; }
-            else if (op == 3) rpos += len;
-            else if (op == 5) { if (i != nc - 1) return false; break; }
-        }
-    }
-    return false;
-}
-
-// the first five counters are vtx_bam_metrics' layout; num_low_base_quality has its own getter (vtx_bam_low_base_quality)
+// the counters in RecordCounter order: the first five are vtx_bam_metrics' layout; num_low_base_quality has its own getter
+// (vtx_bam_low_base_quality)
 struct LocusMetrics { unsigned long long num_reads, num_low_mapq, num_non_primary, num_duplicates, num_not_useful, num_low_base_quality; };
+static_assert(sizeof(LocusMetrics) == kNumCounters * sizeof(unsigned long long), "one counter per RecordCounter");
 
-// ---- 3. one thread per locus: the records it fetches, the four filters (and the base-quality floor); pass 0 counts, pass 1 lists
+// ---- 3. one thread per locus: the records it fetches, the record filters (drop_reason); pass 0 counts, pass 1 lists
 __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const int64_t* l_start, const int64_t* l_end, uint32_t n_rec,
                                             const uint64_t* rec_off, const int32_t* rec_tid, const int32_t* rec_pos, const int32_t* rec_end,
                                             const uint32_t* rec_fm, const uint32_t* max_span, uint32_t* max_read, int pass, uint32_t* cand_count,
                                             const uint32_t* cand_first, uint32_t* cand_rec, uint32_t* used, LocusMetrics* met,
-                                            uint32_t* lfilt = nullptr /* pass 0, vtx_set_locus_stats: [l][6] the counters below */)
+                                            uint32_t* lfilt = nullptr /* pass 0, vtx_set_locus_stats: [l][kNumCounters] */)
 {
     const int64_t start = l_start[l], end = l_end[l];
     // records are coordinate-sorted: candidates lie in [first pos > start - max_span, first pos >= end)
@@ -177,17 +137,17 @@ __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const i
     while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (int64_t(rec_pos[mid]) < end) lo = mid + 1; else hi = mid; }
     const uint32_t last = lo;
     uint32_t n = 0, longest = 0;
-    unsigned long long fetched = 0, low = 0, nonprim = 0, dup = 0, notuse = 0, lowbq = 0;
+    uint32_t c[kNumCounters] = {};
     const uint32_t base = pass ? cand_first[l] : 0;
     for (uint32_t i = first; i < last; ++i) {
         if (rec_tid[i] != P.tid || int64_t(rec_end[i]) <= start) continue;
-        ++fetched;                                                                        // main.rs:831
-        const uint32_t fm = rec_fm[i], fl = fm >> 8;
-        if ((fm & 0xFF) < P.mapq_min) { ++low; continue; }                                // 833
-        if (P.primary_only && (fl & 0x900)) { ++nonprim; continue; }                      // 841
-        if (P.no_duplicates && (fl & 0x400)) { ++dup; continue; }                         // 849
-        if (!useful_alignment(P.s + rec_off[i] + 4, start, end)) { ++notuse; continue; }  // 857
-        if (P.min_base_quality && !base_quality_ok(P.s + rec_off[i] + 4, start, end, P.min_base_quality)) { ++lowbq; continue; }
+        ++c[kFetched];                                                                    // main.rs:831
+        const uint32_t fm = rec_fm[i];
+        const int drop = drop_reason(fm >> 8, fm & 0xFF, P.s + rec_off[i] + 4, start, end, P);
+        if (drop) {
+            for (int k = kLowMapq; k < kNumCounters; ++k) c[k] += drop == k;      // constant indices: c stays in registers
+            continue;
+        }
         if (pass) { cand_rec[base + n] = i; used[i] = 1u; }
         else { const uint32_t ls = ld32(P.s + rec_off[i] + 4 + 16); if (ls > longest) longest = ls; }                       // l_seq of a read that will be scored
         ++n;
@@ -195,65 +155,15 @@ __host__ __device__ inline void locus_cands(const Params& P, uint32_t l, const i
     if (!pass) {
         cand_count[l] = n;
         if (longest) take_max(max_read, longest);
-        if (fetched) add_u64(&met->num_reads, fetched);
-        if (low) add_u64(&met->num_low_mapq, low);
-        if (nonprim) add_u64(&met->num_non_primary, nonprim);
-        if (dup) add_u64(&met->num_duplicates, dup);
-        if (notuse) add_u64(&met->num_not_useful, notuse);
-        if (lowbq) add_u64(&met->num_low_base_quality, lowbq);
-        if (lfilt) {                     // the per-locus split of the same counters (vtx_locus_stats.cuh)
-            uint32_t* f = lfilt + size_t(l) * 6;
-            f[0] = uint32_t(fetched); f[1] = uint32_t(low); f[2] = uint32_t(nonprim); f[3] = uint32_t(dup); f[4] = uint32_t(notuse); f[5] = uint32_t(lowbq);
-        }
+        if (c[kFetched]) add_u64(&met->num_reads, c[kFetched]);
+        if (c[kLowMapq]) add_u64(&met->num_low_mapq, c[kLowMapq]);
+        if (c[kNonPrimary]) add_u64(&met->num_non_primary, c[kNonPrimary]);
+        if (c[kDuplicate]) add_u64(&met->num_duplicates, c[kDuplicate]);
+        if (c[kNotUseful]) add_u64(&met->num_not_useful, c[kNotUseful]);
+        if (c[kLowBaseQuality]) add_u64(&met->num_low_base_quality, c[kLowBaseQuality]);
+        if (lfilt)                       // the per-locus split of the same counters (vtx_locus_stats.cuh)
+            for (int k = 0; k < kNumCounters; ++k) lfilt[size_t(l) * kNumCounters + k] = c[k];
     }
-}
-
-// first aux field named (t0, t1): its value bytes when the type is Z (Record::aux -> Aux::String), else nothing
-__host__ __device__ inline bool aux_z(const uint8_t* p, const uint8_t* e, uint8_t t0, uint8_t t1, uint32_t* off_from_p, uint32_t* len)
-{
-    const uint8_t* base = p;
-    while (p + 3 <= e) {
-        const bool hit = p[0] == t0 && p[1] == t1;
-        const uint8_t ty = p[2];
-        p += 3;
-        if (ty == 'Z' || ty == 'H') {
-            const uint8_t* q = p;
-            while (q < e && *q) ++q;
-            if (q >= e) return false;
-            if (hit) { if (ty == 'Z') { *off_from_p = uint32_t(p - base); *len = uint32_t(q - p); return true; } return false; }
-            p = q + 1;
-        } else {
-            size_t sz;
-            switch (ty) {
-            case 'A': case 'c': case 'C': sz = 1; break;
-            case 's': case 'S': sz = 2; break;
-            case 'i': case 'I': case 'f': sz = 4; break;
-            case 'B': {
-                if (p + 5 > e) return false;
-                const uint8_t sub = p[0]; const uint32_t cnt = ld32(p + 1);
-                const size_t es = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : 4;
-                sz = 5 + size_t(cnt) * es; break;
-            }
-            default: return false;
-            }
-            if (hit) return false;
-            p += sz;
-        }
-    }
-    return false;
-}
-
-// vtx_pack_umi on the device: strings over {A,C,G,T,N} up to 18 bases; anything else cannot be keyed here
-__host__ __device__ inline uint64_t pack_umi(const uint8_t* s, uint32_t len)
-{
-    if (len > 18) return kNoUmi;
-    uint64_t k = 0;
-    for (uint32_t i = 0; i < len; ++i) {
-        uint64_t c;
-        switch (s[i]) { case 'A': c = 0; break; case 'C': c = 1; break; case 'G': c = 2; break; case 'T': c = 3; break; case 'N': c = 4; break; default: return kNoUmi; }
-        k = (k << 3) | c;
-    }
-    return (k << 5) | len;
 }
 
 // ---- 4. one thread per record: the read arrays of the engine -----------------------------------------------------------------
