@@ -59,7 +59,7 @@ template <int S> struct FoldRing {
     uint32_t count[S];               // tiles in flight on the slot
     uint32_t ready[S];               // the slot's tables are built
     uint32_t tag[S];                 // locus the slot holds (kFoldNoTile: none yet)
-    uint32_t mids[S];                // allele columns of that locus: mid_ref | mid_alt << 16
+    uint32_t mids[S];                // that locus's allele columns and shared extension: mid_ref | mid_alt << 8 | x << 16
 };
 
 struct FoldTake {

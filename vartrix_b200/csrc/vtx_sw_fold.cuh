@@ -19,16 +19,22 @@
 //               m - 1 - i, so the per-locus profile is pre-merged over the pair of their codes (25 rows): per
 //               step a lane loads one pair code and its 12 substitution words (3 LDS.128), nothing to merge.
 //               The last column (H + gap, E) of every row goes to shared memory.
-//   middle      the n - 192 allele columns (9 for an SNV with --padding 100, up to 40): halves are (ref, alt)
-//               again.  Lane g owns the 19 read rows [19 g, 19 g + 19), whose (H + gap, E) start from the parked
-//               forward boundary, and the 8 lanes of a unit walk over the columns together, one column per step:
-//               F down a column is a running maximum, so it crosses the lanes as one exclusive max-scan.
+//   extension   the flanks of a window usually reach past 96 columns (--padding 100: 100 on either side of an SNV),
+//               so the columns between the main pass and the allele columns are common to ref and alt too.  The
+//               table builder picks x (both sides the same, 0 when nothing more is shared): the halves stay
+//               (forward, reversed), continued over hap[96, 96 + x) and reversed hap[n - 96 - x, n - 96) once for
+//               both haplotypes, column-synchronously like the allele columns below.  Its reversed boundary
+//               replaces the parked one.  An SNV with --padding 100 has 4 + 1 such column steps instead of 9.
+//   middle      the remaining n - 192 - 2 x allele columns (up to 40): halves are (ref, alt) again.  Lane g owns
+//               the 19 read rows [19 g, 19 g + 19), whose (H + gap, E) start from the forward boundary, and the 8
+//               lanes of a unit walk over the columns together, one column per step: F down a column is a running
+//               maximum, so it crosses the lanes as one exclusive max-scan.
 //   junction    after the last allele column of a haplotype every lane adds the parked reverse boundary of the
 //               partner rows (reversed row m - 2 - r for forward row r).
 //
-// Per pair this is 2 x 96 + (n - 192) column-passes in "one read per word" units instead of 96 / 2 + (n - 96):
-// ~25 % fewer DPX instructions than vtx_k_sw_split for an SNV window.  Reads up to kFoldMaxRead bases,
-// windows with both flanks >= 96 columns in common and at most kFoldMaxMid allele columns.
+// Per pair this is 2 x (96 + x) + (n - 192 - 2 x) column-passes in "one read per word" units instead of
+// 96 / 2 + (n - 96): ~25 % fewer DPX instructions than vtx_k_sw_split for an SNV window.  Reads up to kFoldMaxRead
+// bases, windows with both flanks >= 96 columns in common and at most kFoldMaxMid allele columns.
 #pragma once
 #include <cuda/atomic>
 #include "vtx_sw.cuh"
@@ -66,8 +72,10 @@ constexpr int kFoldUnroll = VTX_FOLD_UNROLL;         // row-loop unrolling of th
 #endif
 constexpr int kFoldMidUnroll = VTX_FOLD_MID_UNROLL;  // column-loop unrolling of the allele pass
 
-// per-locus slot: merged profile [pair code][column], then the allele-column table [column][read code]
-constexpr size_t kFoldSlotBytes = (size_t(kFoldPairRows) * kFoldP + size_t(kFoldMaxMid) * 8) * 4;
+// per-locus slot: merged profile [pair code][column], then kFoldMidTabBytes for the shared-extension table
+// [column][pair code] (kFoldExtColBytes per column) followed by the allele-column table [column][read code] (32 bytes)
+constexpr int kFoldMidTabBytes = kFoldMaxMid * 32, kFoldExtColBytes = kFoldPairRows * 4;
+constexpr size_t kFoldSlotBytes = size_t(kFoldPairRows) * kFoldP * 4 + kFoldMidTabBytes;
 // per warp: boundary column (forward | reverse) per read and row, then the row codes (forward, and pair (row i, row m - 1 - i))
 constexpr size_t kFoldWarpBytes = size_t(kFoldPPW) * kFoldRows * 8 + 32 + size_t(2 * kFoldPPW) * kFoldCodeStride;
 static_assert(kFoldSlotBytes % 16 == 0 && kFoldWarpBytes % 16 == 0, "slots and warp areas stay 16-byte aligned");
@@ -199,7 +207,6 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
             const uint8_t* ah = a.hap_bytes + __ldg(a.alt_off + locus);
             const int n_ref = int(__ldg(a.ref_len + locus)), n_alt = int(__ldg(a.alt_len + locus));
             const int mid_ref = n_ref - 2 * P, mid_alt = n_alt - 2 * P;
-            if (lane == 0) ring.mids[slot] = uint32_t(mid_ref) | uint32_t(mid_alt) << 16;
             // row 5 a + b, column c: {s(a, hap[c]), s(b, hap[n - 1 - c])}; both flanks are common to ref and alt
             // (vtx_k_locus_prep).  Lane j < 24 fills columns [4 j, 4 j + 4) of every row with one STS.128 each.
             if (lane < P / 4) {
@@ -220,20 +227,39 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
                         reinterpret_cast<uint4*>(prof + (5 * ra + rb) * RS1)[lane] = make_uint4(w[0], w[1], w[2], w[3]);
                     }
             }
-            const int lmax = max(mid_ref, mid_alt);
-            for (int idx = lane; idx < lmax * 8; idx += 32) {
+            // x: the columns P + j (left) and n - 1 - P - j (right) that ref and alt still share, j < x.  Both halves
+            // extend by the same x (a half cannot be padded with sentinel columns without changing its boundary), every
+            // allele keeps at least one column of its own (the junction follows them), and both tables fit the slot.
+            const int lmax = max(mid_ref, mid_alt), lmin = min(mid_ref, mid_alt);
+            const int x_cap = min((lmin - 1) / 2, (kFoldMidTabBytes - 32 * lmax) / (kFoldExtColBytes - 64));
+            const bool shared = lane < x_cap && __ldg(rh + P + lane) == __ldg(ah + P + lane) &&
+                                __ldg(rh + (n_ref - 1 - P - lane)) == __ldg(ah + (n_alt - 1 - P - lane));
+            const int x = __ffs(~__ballot_sync(0xffffffffu, shared)) - 1;
+            const int am_ref = mid_ref - 2 * x, am_alt = mid_alt - 2 * x;
+            if (lane == 0) ring.mids[slot] = uint32_t(am_ref) | uint32_t(am_alt) << 8 | uint32_t(x) << 16;
+            // shared extension [column][pair code]: the main pass's merged profile continued over columns P + j, lane j
+            // filling column j
+            if (lane < x) {
+                const uint32_t fb = hap_code(__ldg(rh + P + lane)), sb = hap_code(__ldg(rh + (n_ref - 1 - P - lane)));
+#pragma unroll
+                for (uint32_t ra = 0; ra < 5; ++ra)
+#pragma unroll
+                    for (uint32_t rb = 0; rb < 5; ++rb)
+                        midtab[lane * kFoldPairRows + 5 * ra + rb] = pack2(ra == fb ? kProfMatch : kProfMis, rb == sb ? kProfMatch : kProfMis);
+            }
+            uint32_t* alltab = midtab + x * kFoldPairRows;
+            for (int idx = lane; idx < (lmax - 2 * x) * 8; idx += 32) {
                 const int k = idx >> 3;
                 const uint32_t r = uint32_t(idx & 7);
-                const uint32_t rb = k < mid_ref ? hap_code(__ldg(rh + P + k)) : 5u;      // past the shorter allele: sentinel
-                const uint32_t ab = k < mid_alt ? hap_code(__ldg(ah + P + k)) : 5u;
-                midtab[idx] = pack2(r == rb ? kProfMatch : kProfMis, r == ab ? kProfMatch : kProfMis);
+                const uint32_t rb = k < am_ref ? hap_code(__ldg(rh + P + x + k)) : 5u;   // past the shorter allele: sentinel
+                const uint32_t ab = k < am_alt ? hap_code(__ldg(ah + P + x + k)) : 5u;
+                alltab[idx] = pack2(r == rb ? kProfMatch : kProfMis, r == ab ? kProfMatch : kProfMis);
             }
             __syncwarp();
             if (SHARED && lane == 0) ring_publish<FoldSyncDev>(ring, slot);
         } else if (SHARED) {
             ring_wait<FoldSyncDev>(ring, slot);                          // every lane acquires the builder's tables
         }
-        const int mid_ref = int(ring.mids[slot] & 0xFFFFu), mid_alt = int(ring.mids[slot] >> 16);
         // ---- row codes: the 8 lanes of a unit fill their read's forward codes, then the pair codes from them ----
         const uint32_t pair = p0 + u;
         const bool active = pair < p_end;
@@ -319,22 +345,20 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
         }
         __syncwarp();
 
-        // =========================== middle: (ref, alt) over the allele columns, rows in registers ===========================
+        // ============ shared extension: (forward, reversed) again; middle: (ref, alt) over the allele columns ============
         {
-            const int lmax = max(mid_ref, mid_alt), lmin = min(mid_ref, mid_alt);
-            // the half whose allele ends first, and its last column (none for equal alleles)
-            const uint32_t short_mask = mid_ref < mid_alt ? 0x0000FFFFu : mid_alt < mid_ref ? 0xFFFF0000u : 0u;
-            const int k_short = lmin != lmax ? lmin - 1 : -1;
+            const uint32_t mids = ring.mids[slot];                               // read here: nothing held across the main pass
             uint32_t hg[R], e[R], rc[R];
+            const uint8_t* cpm = cp + M + R * g;
             const uint8_t* cfm = cf + M + R * g;
 #pragma unroll
             for (int c = 0; c < R; ++c) {
                 const int row = R * g + c;
                 uint2 b = make_uint2(kGOE2, kNEG2);
                 if (row < mmax) b = row_bnd[row];
-                hg[c] = __byte_perm(b.x, 0, 0x1010);                             // forward half, for ref and alt
-                e[c] = __byte_perm(b.y, 0, 0x1010);
-                rc[c] = uint32_t(cfm[c]) * 4u;
+                hg[c] = b.x;                                                     // (forward, reversed) as parked
+                e[c] = b.y;
+                rc[c] = uint32_t(cpm[c]) * 4u;                                   // pair code of forward row r, reversed row r
             }
             // junction of the halves in `mask`: forward row r meets reversed row m - 2 - r
             // (one base register and the row's constant offset, not one row index per c held across the allele pass)
@@ -364,12 +388,10 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
             // a(r') for some r' < r), so `best` takes a.
             // Ranges: a is biased in [kBias, kBias + 152], y in [kBias, kBias + 152 + 151] once offset, P never below
             // kScanNeg2 - 19 * 7: all halves stay far inside int16 and above every negative constant added to them below.
-            const uint8_t* tab = reinterpret_cast<const uint8_t*>(midtab);
-#pragma unroll kFoldMidUnroll
-            for (int k = 0; k < lmax; ++k) {
-                const uint8_t* trow = tab + 32 * k;                              // midtab[k][*]
-                // H(19 g - 1, k - 1) + goe: the last row of the lane above, before pass 1 overwrites it (at k = 0 the
-                // parked forward boundary); row -1 of the matrix is H = 0
+            // One column of both halves; trow is the column's table row, indexed by rc.
+            auto column = [&](const uint8_t* trow) {
+                // H(19 g - 1, k - 1) + goe: the last row of the lane above, before pass 1 overwrites it (at the first
+                // column the parked boundary); row -1 of the matrix is H = 0
                 uint32_t diag = __shfl_up_sync(0xffffffffu, hg[R - 1], 1, 8);
                 if (g == 0) diag = kGOE2;
                 uint32_t aa[2], yy[2], ymax = kBIAS2;                            // y >= kBias: the floor changes nothing
@@ -407,6 +429,32 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
                     hg[c] = __viaddmax_s16x2(p, kGO2, yv) + fold_row_hg_add(c);
                     if (c + 1 < R) p = __vmaxs2(p, yv);
                 }
+            };
+            // Shared extension: columns [P, P + x) forward and [n - P - x, n - P) reversed, common to ref and alt, so
+            // scored once for both (the table builder chose x).  Forward row r and reversed row r are read rows r and
+            // m - 1 - r, so the table is indexed by pair code like the main pass's profile.
+            const uint8_t* tab = reinterpret_cast<const uint8_t*>(midtab);
+            for (int k = int(mids >> 16); k > 0; --k, tab += kFoldExtColBytes) column(tab);
+            best = __vmaxs2(best, __byte_perm(best, 0, 0x1032));                 // both halves count for ref and alt
+            // park the extended reversed boundary for the junction; the allele columns continue the forward half.  Rows
+            // 149..151 land on scratch entries (see above), so every row is stored.
+            uint2* park = my_bnd + 7 + R * g;
+#pragma unroll
+            for (int c = 0; c < R; ++c) {
+                park[c] = make_uint2(hg[c], e[c]);
+                hg[c] = __byte_perm(hg[c], 0, 0x1010);
+                e[c] = __byte_perm(e[c], 0, 0x1010);
+                rc[c] = uint32_t(cfm[c]) * 4u;
+            }
+            __syncwarp();                                                        // the junction reads other lanes' rows
+            const int mid_ref = int(mids & 0xFFu), mid_alt = int((mids >> 8) & 0xFFu);
+            const int lmax = max(mid_ref, mid_alt), lmin = min(mid_ref, mid_alt);
+            // the half whose allele ends first, and its last column (none for equal alleles)
+            const uint32_t short_mask = mid_ref < mid_alt ? 0x0000FFFFu : mid_alt < mid_ref ? 0xFFFF0000u : 0u;
+            const int k_short = lmin != lmax ? lmin - 1 : -1;
+#pragma unroll kFoldMidUnroll
+            for (int k = 0; k < lmax; ++k) {
+                column(tab + 32 * k);                                            // allele table [k][*]
                 if (k == k_short) junction(short_mask);                          // the shorter allele ends here (indels only)
             }
             junction(~short_mask);                                                // every lane has finished column lmax - 1
