@@ -12,7 +12,7 @@
 using namespace vtx;
 
 template <int LEVEL>
-__global__ void __launch_bounds__(320, 2) k_loop(uint32_t* out, int steps, long long* cyc, uint32_t k64k, uint32_t one, const uint8_t* codes_g)
+__global__ void __launch_bounds__(320, 2) k_loop(uint32_t* out, int steps, long long* cyc, uint32_t k64k, const uint8_t* codes_g)
 {
     constexpr int C1 = 12;
     __shared__ __align__(16) uint32_t prof[2 * 5 * 96];                 // forward + reverse profile (shared by the warps: read only)
@@ -73,10 +73,10 @@ __global__ void __launch_bounds__(320, 2) k_loop(uint32_t* out, int steps, long 
                 const int c = 4 * q + k;
                 const uint32_t fc = __viaddmax_s16x2(f[c], kGE2, hg[c]);
                 e = __viaddmax_s16x2(e, kGE2, eg);
-                const uint32_t h = sw_h(diag, one, sv[k], fc, e);
+                const uint32_t h = sw_h(diag, sv[k], fc, e);
                 hh[k] = h;
                 diag = hg[c];
-                hleft = hadd(h, one, c);
+                hleft = h + kGoeAdd;
                 eg = hleft;
                 hg[c] = hleft;
                 f[c] = fc;
@@ -102,8 +102,8 @@ template <int LEVEL> void run(const char* name, const uint8_t* codes)
     int n_sm = 0; cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, 0);
     const int blocks = n_sm * 2, steps = 20000;
     uint32_t* out; long long* cyc; cudaMalloc(&out, size_t(blocks) * 320 * 4); cudaMalloc(&cyc, blocks * 8);
-    k_loop<LEVEL><<<blocks, 320>>>(out, 200, cyc, 65536u, 1u, codes);
-    k_loop<LEVEL><<<blocks, 320>>>(out, steps, cyc, 65536u, 1u, codes);
+    k_loop<LEVEL><<<blocks, 320>>>(out, 200, cyc, 65536u, codes);
+    k_loop<LEVEL><<<blocks, 320>>>(out, steps, cyc, 65536u, codes);
     cudaError_t e = cudaDeviceSynchronize();
     if (e != cudaSuccess) { printf("%s: %s\n", name, cudaGetErrorString(e)); return; }
     static long long h[1024]; cudaMemcpy(h, cyc, blocks * 8, cudaMemcpyDeviceToHost);

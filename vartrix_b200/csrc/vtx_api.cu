@@ -334,22 +334,13 @@ struct DevBatch {   // device pointers
     const uint32_t* cand_read;       // nullptr: candidate c is read c
     // slim layout: cell tags as codes (then cb_bytes / cb_off_ex hold the exotic tags only)
     const uint64_t* read_cb_key = nullptr; const uint32_t* cb_off_ex = nullptr;
-    uint32_t class_mask = ~0u;       // tile classes that may get tiles (host batches: from the windows; device batches: all)
+    bool have_shapes = false;        // host batches: `shapes` holds the shape keys of the loci (scan_host_batch)
+    uint64_t shapes = 0;
     uint32_t max_read_len = 0, max_hap_len = 0;
     uint64_t max_depth = ~0ull;      // most candidates of one locus (unknown for device batches: assume deep)
     const uint32_t* lfilt = nullptr; // [n_loci][stage::kNumCounters] record-filter counters of a vtx_submit_bam shard (vtx_set_locus_stats)
 };
 
-// the allow_* switches of run_sw, shared with the host-side class mask
-struct SwAllow { bool split, multi, fold; };
-SwAllow sw_allow(const vtx_ctx* ctx, uint32_t max_read, uint32_t max_hap)
-{
-    SwAllow a;
-    a.split = max_read <= uint32_t(kSplitMaxRead) && !(ctx->cfg.flags & VTX_F_NO_SPLIT);
-    a.multi = max_read <= uint32_t(kMultiMaxRead) && max_hap > uint32_t(class_max_n(kNumFastClasses - 1));
-    a.fold = !(ctx->cfg.flags & (VTX_F_NO_SPLIT | VTX_F_NO_FOLD));
-    return a;
-}
 // A persistent grid of a Smith-Waterman kernel: as many blocks as fit on every SM at once, each warp taking tiles from
 // a.tile_counter until none are left.  `name` / `cls` (-1: none) name the kernel in the error message.
 int launch_sw(vtx_ctx* ctx, void (*kern)(SwArgs), int threads, size_t smem, const SwArgs& a, uint64_t* launches,
@@ -393,11 +384,10 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
     ENS(ctx->tcount, size_t(kNumClasses) * (nl + 1) * 4);
     ENS(ctx->tstart, size_t(kNumClasses) * (nl + 1) * 4);
     ENS(ctx->tile_counters, 64);
-    const SwAllow allow = sw_allow(ctx, b.max_read_len, b.max_hap_len);     // fold: per locus, windows and read lengths decide
+    const SwAllow allow = allowed_kernels(ctx->cfg.flags, b.max_read_len, b.max_hap_len);
     vtx_k_locus_prep<<<blocks_for(uint64_t(nl) * 32, 256), 256, 0, ctx->stream>>>(
         nl, b.hap, b.ref_off, b.ref_len, b.alt_off, b.alt_len, P<uint32_t>(ctx->pair_start), P<uint32_t>(ctx->pair_read), b.read_len,
-        /*force_slow=*/0, allow.split, allow.multi, allow.fold, b.max_read_len, b.max_hap_len, P<unsigned long long>(ctx->d_metrics) + 4,
-        P<uint32_t>(ctx->tcount));
+        allow, b.max_read_len, b.max_hap_len, P<unsigned long long>(ctx->d_metrics) + 4, P<uint32_t>(ctx->tcount));
     ++*launches;
     vtx_k_scan_rows<<<kNumClasses, kScanThreads, 0, ctx->stream>>>(P<uint32_t>(ctx->tcount), P<uint32_t>(ctx->tstart), nl, nl + 1);
     ++*launches;
@@ -417,7 +407,6 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
     mcap = std::max(2, (mcap + 1) & ~1);
     a.mcap = mcap;
     a.k64k = 65536u;
-    a.one = 1u;
     a.multi = allow.multi;
     a.max_hap = b.max_hap_len;
 
@@ -447,12 +436,10 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
         *sw_launches += *launches - before;
         return VTX_OK;
     }
-    // b.class_mask: for host batches the classes the windows of this shard can select (scan_host_batch); all for device batches
-    for (int c = 0; c < kNumFastClasses; ++c) {
-        // a class whose narrowest window is wider than every window of this batch has no tiles: skip the empty launch
-        // (max_hap_len is exact for host batches and a promised upper bound for device batches)
-        if (c > 0 && b.max_hap_len <= uint32_t(class_max_n(c - 1))) continue;
-        if (!(b.class_mask >> c & 1u)) continue;
+    // the kernels of the classes that can get tiles: from the loci's shapes when the host has seen them
+    const uint32_t mask = b.have_shapes ? host_class_mask(b.shapes, allow, b.max_read_len) : device_class_mask(allow, b.max_hap_len);
+    for (int c = 0; c < kNumClasses; ++c) {
+        if (!(mask >> c & 1u)) continue;
         a.tile_start = P<uint32_t>(ctx->tstart) + size_t(c) * (nl + 1);
         a.tile_counter = P<uint32_t>(ctx->tile_counters) + c;
         int rc = VTX_OK;
@@ -461,40 +448,29 @@ int run_sw(vtx_ctx* ctx, const DevBatch& b, uint32_t n_pairs_ub, const uint32_t*
         case 1: rc = launch_sw_class<1>(ctx, a, launches); break;
         case 2: rc = launch_sw_class<2>(ctx, a, launches); break;
         case 3: rc = launch_sw_class<3>(ctx, a, launches); break;
+        case kSlowClass: {
+            const unsigned blocks = unsigned(ctx->n_sm) * 4, threads = 128;
+            const size_t warps = size_t(blocks) * threads / 32;
+            ENS(ctx->scratch, warps * (size_t(b.max_hap_len) + 1) * 32 * 4);
+            a.scratch = P<uint32_t>(ctx->scratch);
+            vtx_k_sw_generic<<<blocks, threads, 0, ctx->stream>>>(a);
+            CK(cudaGetLastError());
+            ++*launches;
+            break;
         }
-        if (rc) return rc;
-    }
-    if (allow.split) {
-        for (int c = 0; c < kNumSplitClasses; ++c) {
-            if (c > 0 && b.max_hap_len <= uint32_t(split_max_n(c - 1))) continue;
-            if (!(b.class_mask >> (kSplitClass0 + c) & 1u)) continue;
-            a.tile_start = P<uint32_t>(ctx->tstart) + size_t(kSplitClass0 + c) * (nl + 1);
-            a.tile_counter = P<uint32_t>(ctx->tile_counters) + kSplitClass0 + c;
-            int rc = c == 0 ? launch_sw_split<0>(ctx, a, launches) : launch_sw_split<1>(ctx, a, launches);
-            if (rc) return rc;
-        }
-    }
-    if (allow.fold && (b.class_mask >> kFoldClass & 1u)) {
-        a.tile_start = P<uint32_t>(ctx->tstart) + size_t(kFoldClass) * (nl + 1);
-        a.tile_counter = P<uint32_t>(ctx->tile_counters) + kFoldClass;
-        // the depth is taken over all candidates and loci of the shard, which the host knows for host and device
-        // batches alike, not over fold tiles: shallow fold loci in a shard of deep loci of other kernels run the deep
-        // shape, which is slower on 1-tile loci but still exact
-        const bool deep = uint64_t(n_pairs_ub) >= uint64_t(kFoldDeepDepth) * nl;
-        int rc = deep ? launch_sw_fold<kFoldDeepWarps, kFoldDeepSlots, true>(ctx, a, launches)
+        case kSplitClass0: rc = launch_sw_split<0>(ctx, a, launches); break;
+        case kSplitClass0 + 1: rc = launch_sw_split<1>(ctx, a, launches); break;
+        case kFoldClass: {
+            // the depth is taken over all candidates and loci of the shard, which the host knows for host and device
+            // batches alike, not over fold tiles: shallow fold loci in a shard of deep loci of other kernels run the deep
+            // shape, which is slower on 1-tile loci but still exact
+            const bool deep = uint64_t(n_pairs_ub) >= uint64_t(kFoldDeepDepth) * nl;
+            rc = deep ? launch_sw_fold<kFoldDeepWarps, kFoldDeepSlots, true>(ctx, a, launches)
                       : launch_sw_fold<kFoldShallowWarps, kFoldShallowWarps, false>(ctx, a, launches);
+            break;
+        }
+        }
         if (rc) return rc;
-    }
-    if (b.class_mask >> kSlowClass & 1u) {   // generic class (rare)
-        const unsigned blocks = unsigned(ctx->n_sm) * 4, threads = 128;
-        const size_t warps = size_t(blocks) * threads / 32;
-        ENS(ctx->scratch, warps * (size_t(b.max_hap_len) + 1) * 32 * 4);
-        a.scratch = P<uint32_t>(ctx->scratch);
-        a.tile_start = P<uint32_t>(ctx->tstart) + size_t(kSlowClass) * (nl + 1);
-        a.tile_counter = P<uint32_t>(ctx->tile_counters) + kSlowClass;
-        vtx_k_sw_generic<<<blocks, threads, 0, ctx->stream>>>(a);
-        CK(cudaGetLastError());
-        ++*launches;
     }
     *sw_launches += *launches - before;
     return VTX_OK;
@@ -816,51 +792,10 @@ int validate_batch(vtx_ctx* ctx, const BatchView& b)
     return VTX_OK;
 }
 
-// Which Smith-Waterman tile classes can get tiles, from the windows alone: the same decision tree as vtx_k_locus_prep,
-// with the one input the host does not have (the longest SCORED read of a fold-shaped locus) resolved conservatively.
-// Index of the per-locus shape: bit 0 exotic, bit 1 common prefix, bit 2 fold-shaped windows, bits 3.. single-phase
-// class (kNumFastClasses = none), then the two-phase class (kNumSplitClasses = none).
-constexpr int kShapeFast = 3, kShapeSplit = kShapeFast + 3, kNumShapes = 1 << (kShapeSplit + 2);
-uint32_t shape_of(const uint8_t* rh, uint32_t nr, const uint8_t* ah, uint32_t na)
-{
-    // The alphabet test of vtx_k_locus_prep ("=MRSVWYHKDBN" bytes send a locus to the generic kernel) is not repeated on
-    // the host -- a byte-wise scan of every window would cost more than the launch it can save: the generic class is
-    // always launched, and bit 0 stays clear.
-    const bool same = nr >= uint32_t(kSplitP) && na >= uint32_t(kSplitP) && memcmp(rh, ah, kSplitP) == 0;
-    const bool fold = same && std::min(nr, na) > uint32_t(2 * kFoldP) && std::max(nr, na) <= uint32_t(2 * kFoldP + kFoldMaxMid) &&
-                      memcmp(rh + nr - kFoldP, ah + na - kFoldP, kFoldP) == 0;
-    const uint32_t nmax = std::max(nr, na);
-    uint32_t fast = kNumFastClasses, split = kNumSplitClasses;
-    for (int c = kNumFastClasses - 1; c >= 0; --c) if (nmax <= uint32_t(class_max_n(c))) fast = uint32_t(c);
-    for (int c = kNumSplitClasses - 1; c >= 0; --c) if (nmax <= uint32_t(split_max_n(c))) split = uint32_t(c);
-    return (uint32_t(same) << 1) | (uint32_t(fold) << 2) | (fast << kShapeFast) | (split << kShapeSplit);
-}
-uint32_t class_mask_of(const bool* seen, bool allow_split, bool allow_multi, bool allow_fold, uint32_t max_read)
-{
-    uint32_t mask = 1u << kSlowClass;          // loci with IUPAC / "=" bytes are only recognised on the device
-    for (int i = 0; i < kNumShapes; ++i) {
-        if (!seen[i]) continue;
-        const bool exotic = i & 1, same = i & 2, fold = i & 4;
-        const uint32_t fast = (uint32_t(i) >> kShapeFast) & 7u, split = (uint32_t(i) >> kShapeSplit) & 3u;
-        int cls = kSlowClass;
-        if (!exotic) {
-            if (fast < uint32_t(kNumFastClasses)) cls = int(fast);
-            else if (allow_multi) cls = kMultiClass;
-            if (same && allow_split && split < uint32_t(kNumSplitClasses)) cls = kSplitClass0 + int(split);
-            if (fold && allow_fold) {
-                mask |= 1u << kFoldClass;
-                if (max_read <= uint32_t(kFoldMaxRead)) continue;        // every read fits: the locus cannot fall back
-            }
-        }
-        mask |= 1u << cls;
-    }
-    return mask;
-}
-
 // host-side checks that need to touch the (host) arrays; also returns max lengths.  Runs on a few host
 // threads while the shard's H2D copies are already in flight (the kernels are only enqueued afterwards).
 int scan_host_batch(vtx_ctx* ctx, const BatchView& b, uint32_t* max_read, uint32_t* max_hap, bool check_cands,
-                    uint64_t* max_depth = nullptr, bool* shapes_seen = nullptr)
+                    uint64_t* max_depth = nullptr, uint64_t* shapes_seen = nullptr)
 {
     if (check_cands && b.n_loci && (b.cand_start[0] != 0 || b.cand_start[b.n_loci] != b.n_cand))
         return set_err(ctx, VTX_E_INVALID, "cand_start must span [0, n_cand]");
@@ -873,7 +808,7 @@ int scan_host_batch(vtx_ctx* ctx, const BatchView& b, uint32_t* max_read, uint32
     const uint64_t work = uint64_t(b.n_reads) + (scan_cands ? b.n_cand : 0) + uint64_t(b.n_loci) * 64;
     unsigned nt = std::min<unsigned>(8u, std::max(1u, std::thread::hardware_concurrency()));
     if (work < (1u << 16)) nt = 1;
-    struct Part { uint32_t mr = 0, mh = 0; uint64_t md = 0, units = 0; int bad = 0; uint64_t where = 0; bool seen[kNumShapes] = {}; };
+    struct Part { uint32_t mr = 0, mh = 0; uint64_t md = 0, units = 0; int bad = 0; uint64_t where = 0, seen = 0; };
     std::vector<Part> parts(nt);
     auto worker = [&](unsigned t) {
         Part& pt = parts[t];
@@ -886,7 +821,7 @@ int scan_host_batch(vtx_ctx* ctx, const BatchView& b, uint32_t* max_read, uint32
             if (check_cands && b.cand_start[l] > b.cand_start[l + 1]) flag(13, l);
             if (check_cands) pt.md = std::max<uint64_t>(pt.md, b.cand_start[l + 1] - b.cand_start[l]);
             pt.mh = std::max(pt.mh, std::max(b.ref_len[l], b.alt_len[l]));
-            if (shapes_seen) pt.seen[shape_of(b.hap + b.ref_off[l], b.ref_len[l], b.hap + b.alt_off[l], b.alt_len[l])] = true;
+            if (shapes_seen) pt.seen |= uint64_t(1) << shape_key(window_shape(b.hap + b.ref_off[l], b.ref_len[l], b.hap + b.alt_off[l], b.alt_len[l]));
         }
         const uint32_t r0 = uint32_t(uint64_t(b.n_reads) * t / nt), r1 = uint32_t(uint64_t(b.n_reads) * (t + 1) / nt);
         for (uint32_t r = r0; r < r1; ++r) {
@@ -926,7 +861,7 @@ int scan_host_batch(vtx_ctx* ctx, const BatchView& b, uint32_t* max_read, uint32
     uint64_t md = 0, units = 0;
     for (const Part& pt : parts) {
         mr = std::max(mr, pt.mr); mh = std::max(mh, pt.mh); md = std::max(md, pt.md); units += pt.units;
-        if (shapes_seen) for (int i = 0; i < kNumShapes; ++i) shapes_seen[i] |= pt.seen[i];
+        if (shapes_seen) *shapes_seen |= pt.seen;
         const unsigned long long w = (unsigned long long)pt.where;
         switch (pt.bad) {
         case 1: return set_err(ctx, VTX_E_INVALID, "read %llu: read_off must be a multiple of 16", w);
@@ -947,12 +882,6 @@ int scan_host_batch(vtx_ctx* ctx, const BatchView& b, uint32_t* max_read, uint32
     *max_read = mr; *max_hap = mh;
     if (max_depth) *max_depth = md;
     return VTX_OK;
-}
-
-uint32_t host_class_mask(const vtx_ctx* ctx, const bool* shapes, uint32_t max_read, uint32_t max_hap)
-{
-    const SwAllow a = sw_allow(ctx, max_read, max_hap);
-    return class_mask_of(shapes, a.split, a.multi, a.fold, max_read);
 }
 
 int upload(vtx_ctx* ctx, DBuf& d, const void* h, size_t bytes)
@@ -1097,11 +1026,10 @@ int submit_host(vtx_ctx* ctx, const Batch* hb, const char* fn)
     CK(cudaEventRecord(sl->copy_done, ctx->copy_stream));
     tr->had_h2d = true;
     // 2. ... validate the host arrays meanwhile; nothing has been launched on them yet
-    bool shapes[kNumShapes] = {};
     { Nvtx r_val("vtx: validate host batch (copies in flight)");
-      rc = scan_host_batch(ctx, h, &d.max_read_len, &d.max_hap_len, true, &d.max_depth, shapes); }
+      rc = scan_host_batch(ctx, h, &d.max_read_len, &d.max_hap_len, true, &d.max_depth, &d.shapes); }
     if (rc) { cudaStreamSynchronize(ctx->copy_stream); --ctx->trec_used; return rc; }
-    d.class_mask = host_class_mask(ctx, shapes, d.max_read_len, d.max_hap_len);
+    d.have_shapes = true;
     // 3. kernels wait for the copy, and release the slot when done
     CK(cudaStreamWaitEvent(ctx->stream, sl->copy_done, 0));
     CK(cudaEventRecord(tr->ev[EV_C0], ctx->stream));

@@ -328,9 +328,6 @@ __host__ __device__ inline int decode_batch(State& s, Tables& T, uint8_t* lens, 
 // dependent ALU and shared-memory operations, so a warp takes milliseconds per 64 KB member -- and what buys throughput is
 // the number of members in flight: 20 warps per SM hide each other's latencies.  The alternative, the member's output
 // assembled in 64 KB of shared memory by a lone warp per CTA, is faster per member but fits only 2 CTAs on an SM.
-#ifndef VTX_INFLATE_PIPELINE
-#define VTX_INFLATE_PIPELINE 1
-#endif
 constexpr int kInflateWarps = 4;                  // per CTA
 constexpr int kBatch = 32;
 
@@ -349,12 +346,8 @@ static_assert(kMaxInputPerCall % 4 == 0 && kInWords * 4 >= 2 * int(kMaxInputPerC
 struct WarpShared {
     Tables T;
     uint8_t lens[512];
-#if VTX_INFLATE_PIPELINE
     Sym batch2[2][kBatch];         // decoded by lane 0 while the other lanes apply the previous one
     int n2[2], done2[2];
-#else
-    Sym batch[kBatch];
-#endif
     uint32_t in_win[kInWords];     // payload words [win_first, win_first + kInWords): the bit reader's refills never leave it
     int n, status, done;
     uint32_t reload;               // first word of the window to load next, or ~0
@@ -435,12 +428,13 @@ __global__ void __launch_bounds__(kInflateWarps * 32) vtx_k_bgzf_inflate(const B
             if (bd.out_len > 65536u || (bd.in_off & 3)) st.status = kBadSize;
             ws.done = 0; ws.reload = 0;
         }
-#if VTX_INFLATE_PIPELINE
         // Lane 0 decodes batch k + 1 while lanes 1..31 apply batch k: the two are latency chains of different kinds (ALU /
         // shared-memory lookups there, L2 round trips of the match copies here) and the divergent halves of the warp are
         // scheduled independently, so they hide each other.  Batches hold at most 31 symbols: one per applying lane.
         uint32_t op = 0;
         constexpr uint32_t kApply = 0xFFFFFFFEu;
+        // the dependent chain of the bit reader runs on shared memory: the warp moves the window when the next call could
+        // leave it (an L2 round trip per ~1 KB of input instead of one per 4 bytes)
         auto load_window = [&]() {                       // all 32 lanes
             __syncwarp();
             const uint32_t reload = ws.reload;
@@ -496,58 +490,6 @@ __global__ void __launch_bounds__(kInflateWarps * 32) vtx_k_bgzf_inflate(const B
             if (last) break;
         }
         __syncwarp();
-#else
-        uint32_t op = 0;
-        for (;;) {
-            // the dependent chain of the bit reader runs on shared memory: the warp moves the window when the next call could
-            // leave it (an L2 round trip per ~1 KB of input instead of one per 4 bytes)
-            __syncwarp();
-            const uint32_t reload = ws.reload;
-            if (reload != 0xFFFFFFFFu) {
-                for (int i = lane; i < kInWords; i += 32) ws.in_win[i] = reload + i < max_word ? __ldg(in_g + reload + i) : 0u;
-                win_first = reload;
-            }
-            __syncwarp();
-            if (lane == 0) {
-                st.in32 = ws.in_win - win_first;                   // in32[word] for word in [win_first, win_first + kInWords)
-                ws.n = st.status == kOk ? decode_batch(st, ws.T, ws.lens, ws.batch, kBatch) : 0;
-                ws.status = st.status; ws.done = (st.phase == 3 || st.status != kOk) ? 1 : 0;
-                // refills of the next call touch words [st.word, st.word + kMaxInputPerCall / 4 + 2)
-                ws.reload = (st.word < win_first || st.word + kMaxInputPerCall / 4 + 2 > win_first + kInWords) ? st.word : 0xFFFFFFFFu;
-            }
-            __syncwarp();
-            const int n = ws.n;
-            // positions: exclusive scan of the symbol lengths
-            Sym sy{ 0, 0, 0 };
-            if (lane < n) sy = ws.batch[lane];
-            uint32_t incl = sy.len;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const uint32_t up = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += up; }
-            const uint32_t my_pos = op + incl - sy.len;
-            const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
-            if (lane < n && sy.kind == 0) o[my_pos] = uint8_t(sy.arg);                   // all literals of the batch at once
-            __syncwarp();
-            uint32_t heavy = __ballot_sync(0xffffffffu, lane < n && sy.kind != 0);       // matches and stored runs, in stream order
-            while (heavy) {
-                const int src_lane = __ffs(heavy) - 1;
-                heavy &= heavy - 1;
-                const uint32_t len = __shfl_sync(0xffffffffu, sy.len, src_lane), arg = __shfl_sync(0xffffffffu, sy.arg, src_lane);
-                const uint32_t kind = __shfl_sync(0xffffffffu, sy.kind, src_lane), pos = __shfl_sync(0xffffffffu, my_pos, src_lane);
-                if (kind == 1) {
-                    const uint8_t* srcp = o + pos - arg;
-                    if (arg >= len) { for (uint32_t i = lane; i < len; i += 32) o[pos + i] = __ldcg(srcp + i); }
-                    else { for (uint32_t i = lane; i < len; i += 32) o[pos + i] = __ldcg(srcp + (i % arg)); }
-                } else {
-                    const uint8_t* srcp = comp + bd.in_off + arg;
-                    for (uint32_t i = lane; i < len; i += 32) o[pos + i] = __ldg(srcp + i);
-                }
-                __syncwarp();
-            }
-            op += total;
-            if (ws.done) break;
-            __syncwarp();
-        }
-#endif
         int stt = ws.status;
         if (stt == kOk && check_crc) {
             __syncwarp();

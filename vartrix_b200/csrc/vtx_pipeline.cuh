@@ -196,12 +196,12 @@ __global__ void vtx_k_pair_start_explicit(uint32_t n_loci, uint32_t n_pairs, con
     pair_start[l] = lo;
 }
 
-// one warp per locus: tile class from haplotype width and alphabet, tiles per class
+// one warp per locus: its shape and longest read, then its tile class (vtx_tile_class.cuh) and tiles
 __global__ void vtx_k_locus_prep(uint32_t n_loci, const uint8_t* __restrict__ hap_bytes,
                                  const uint32_t* __restrict__ ref_off, const uint32_t* __restrict__ ref_len,
                                  const uint32_t* __restrict__ alt_off, const uint32_t* __restrict__ alt_len,
                                  const uint32_t* __restrict__ pair_start, const uint32_t* __restrict__ pair_read,
-                                 const uint32_t* __restrict__ read_len, int force_slow, int allow_split, int allow_multi, int allow_fold,
+                                 const uint32_t* __restrict__ read_len, SwAllow allow,
                                  uint32_t max_read, uint32_t max_hap, unsigned long long* __restrict__ bounds_violated,
                                  uint32_t* __restrict__ tcount /* [kNumClasses][n_loci + 1] */)
 {
@@ -211,56 +211,38 @@ __global__ void vtx_k_locus_prep(uint32_t n_loci, const uint8_t* __restrict__ ha
     const uint32_t nr = ref_len[l], na = alt_len[l];
     const uint8_t* rh = hap_bytes + ref_off[l];
     const uint8_t* ah = hap_bytes + alt_off[l];
+    LocusShape s;
     bool exotic = false;
-    // bytes that a decoded read base other than A/C/G/T could equal: "=MRSVWYHKDBN"
-    auto is_exotic = [](uint8_t b) {
-        return b == '=' || b == 'M' || b == 'R' || b == 'S' || b == 'V' || b == 'W' || b == 'Y' || b == 'H' ||
-               b == 'K' || b == 'D' || b == 'B' || b == 'N';
-    };
     for (uint32_t j = lane; j < nr; j += 32) exotic |= is_exotic(rh[j]);
     for (uint32_t j = lane; j < na; j += 32) exotic |= is_exotic(ah[j]);
-    exotic = __any_sync(0xffffffffu, exotic);
+    s.exotic = __any_sync(0xffffffffu, exotic);
     // is the first kSplitP-column prefix common to both haplotypes?  (construct_haplotypes: same left flank)
-    bool same = nr >= uint32_t(kSplitP) && na >= uint32_t(kSplitP);
+    bool same = prefix_possible(nr, na);
     if (same) for (uint32_t j = lane; j < uint32_t(kSplitP); j += 32) same &= (rh[j] == ah[j]);
-    same = __all_sync(0xffffffffu, same);
+    s.prefix = __all_sync(0xffffffffu, same);
     // ... and the last kFoldP columns (same right flank)?  Then neither flank needs a per-haplotype DP (vtx_sw_fold.cuh).
-    bool fold = same && allow_fold && min(nr, na) > uint32_t(2 * kFoldP) && max(nr, na) <= uint32_t(2 * kFoldP + kFoldMaxMid);
+    bool fold = s.prefix && allow.fold && fold_possible(nr, na);
     if (fold) for (uint32_t j = lane; j < uint32_t(kFoldP); j += 32) fold &= (rh[nr - 1 - j] == ah[na - 1 - j]);
-    fold = __all_sync(0xffffffffu, fold);
+    s.fold = __all_sync(0xffffffffu, fold);
     uint32_t longest = 0;
     for (uint32_t p = pair_start[l] + lane; p < pair_start[l + 1]; p += 32) longest = max(longest, read_len[pair_read[p]]);
     longest = __reduce_max_sync(0xffffffffu, longest);
-    // the folded kernel keeps 8 x 19 read rows in registers: every read of the locus must fit
-    fold = fold && longest <= uint32_t(kFoldMaxRead);
     if (lane != 0) return;
-    const uint32_t nmax = max(nr, na);
+    s.width = max(nr, na);
     // Buffers and kernel shapes were sized from max_read / max_hap (exact for host batches, the caller's promise for
     // device batches).  A locus that breaks the promise gets no tiles -- nothing is read or written out of bounds --
     // and the next vtx_finish reports the violation.
-    if (longest > max_read || nmax > max_hap) {
+    if (longest > max_read || s.width > max_hap) {
         atomicAdd(bounds_violated, 1ull);
 #pragma unroll
         for (int c = 0; c < kNumClasses; ++c) tcount[size_t(c) * (n_loci + 1) + l] = 0u;
         return;
     }
-    int cls = kSlowClass;
-    if (!exotic && !force_slow) {
-#pragma unroll
-        for (int c = kNumFastClasses - 1; c >= 0; --c) if (nmax <= uint32_t(class_max_n(c))) cls = c;
-        if (cls == kSlowClass && allow_multi) cls = kMultiClass;        // wider than 320 columns: several passes
-        if (same && allow_split) {
-#pragma unroll
-            for (int c = kNumSplitClasses - 1; c >= 0; --c) if (nmax <= uint32_t(split_max_n(c))) cls = kSplitClass0 + c;
-        }
-        if (fold) cls = kFoldClass;
-    }
+    const int cls = tile_class(s, allow, longest);
     const uint32_t np = pair_start[l + 1] - pair_start[l];
 #pragma unroll
-    for (int c = 0; c < kNumClasses; ++c) {
-        const uint32_t ppw = (c == kSlowClass) ? uint32_t(kSlowPairsPerWarp) : (c == kFoldClass ? uint32_t(kFoldPPW) : (c > kSlowClass ? uint32_t(kSplitPPW) : 4u));
-        tcount[size_t(c) * (n_loci + 1) + l] = (c == cls) ? (np + ppw - 1) / ppw : 0u;
-    }
+    for (int c = 0; c < kNumClasses; ++c)
+        tcount[size_t(c) * (n_loci + 1) + l] = (c == cls) ? (np + pairs_per_tile(c) - 1) / pairs_per_tile(c) : 0u;
 }
 
 // One CTA per locus: rank every pair's cell (and, with --umi, its (cell, UMI)) among the distinct keys

@@ -24,6 +24,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "vtx_tile_class.cuh"
 
 namespace vtx {
 
@@ -45,58 +46,21 @@ constexpr uint32_t kBIAS2 = pack2(kBias, kBias);                    // biased 0 
 constexpr uint32_t kGOE2 = pack2(kBias + kGoe, kBias + kGoe);       // biased (0 + gap): H = 0 seen through H + go + ge
 constexpr uint32_t kNEG2 = pack2(0, 0);                             // biased -16384 ("minus infinity")
 constexpr uint32_t kGoeAdd = (uint32_t(uint16_t(int16_t(kGoe - 1))) << 16) | uint32_t(uint16_t(int16_t(kGoe)));   // + (gap, gap) incl. the carry
-// Cell update.  1 (default): the diagonal add rides inside VIADDMNMX, x = max(diag + s, F), and the floor of local
-// alignment joins the H maximum, h = VIMNMX3(x, E, 0).  0: round-1 form, tf = VIMNMX3(diag + s, F, 0), h = VIMNMX(tf, E).
+// H = max(diag + s, F, E, 0) of one cell (biased halves; `diag` is stored as H + goe and `s` as s - goe).  The diagonal
+// add rides inside VIADDMNMX, x = max(diag + s, F), and the floor of local alignment joins the H maximum, h = VIMNMX3(x, E, 0).
 // On H100 (profiles/h100_dpx_microbench.txt) 3-input DPX instructions hold the ALU pipe for 2 cycles, the 2-input VIMNMX
-// for 1, and a plain add next to a DPX instruction is free -- so form 1 costs 12 more ALU cycles per main-pass step of the
-// folded kernel (126 instead of 114) but 5 fewer issue slots (117 instead of 122); the kernel is bound by both.
-#ifndef VTX_SW_FUSE
-#define VTX_SW_FUSE 1
-#endif
-// The remaining plain add of a cell, H + gap.  ptxas places a plain `x + c` on the ALU pipe (VIADD), which the DPX
-// instructions already saturate; written as x * one + c with a run-time `one` it is an IMAD on the FMA pipe instead.
-// VTX_SW_HADD: 0 = plain add everywhere, 1 = IMAD everywhere, 2 = IMAD on even columns (splits the adds between the pipes).
-#ifndef VTX_SW_HADD
-#define VTX_SW_HADD 0
-#endif
-__device__ __forceinline__ uint32_t padd(uint32_t x, uint32_t one, uint32_t c)
+// for 1, and a plain add next to a DPX instruction is free -- so this form costs 12 more ALU cycles per main-pass step of
+// the folded kernel than the unfused one, max(VIMNMX3(diag + s, F, 0), E) (126 instead of 114), but takes 5 fewer issue
+// slots (117 instead of 122); the kernel is bound by both.
+__device__ __forceinline__ uint32_t sw_h(uint32_t diag, uint32_t s, uint32_t f, uint32_t e)
 {
-    (void)one;
-    return x + c;
-}
-__device__ __forceinline__ uint32_t hadd(uint32_t h, uint32_t one, int col)
-{
-#if VTX_SW_HADD == 1
-    (void)col;
-    return h * one + kGoeAdd;
-#elif VTX_SW_HADD == 2
-    return (col & 1) ? h + kGoeAdd : h * one + kGoeAdd;
-#else
-    (void)one; (void)col;
-    return h + kGoeAdd;
-#endif
-}
-// H = max(diag + s, F, E, 0) of one cell (biased halves; `diag` is stored as H + goe and `s` as s - goe)
-__device__ __forceinline__ uint32_t sw_h(uint32_t diag, uint32_t one, uint32_t s, uint32_t f, uint32_t e)
-{
-#if VTX_SW_FUSE
-    (void)one;
     return __vimax3_s16x2(__viaddmax_s16x2(diag, s, f), e, kBIAS2);
-#else
-    return __vmaxs2(__vimax3_s16x2(padd(diag, one, s), f, kBIAS2), e);
-#endif
 }
 // profile entries are biased by -kGoe because the stored state is H + kGoe
 constexpr int kProfMatch = kMatch - kGoe, kProfMis = kMismatch - kGoe;     // 7, 1
 
 constexpr int kFastMaxRead = 1024;       // row-code buffer of the single-phase kernels; longer reads are scored in row blocks
 constexpr int kMaxRead = 16000;          // biased int16: H + 16384 must stay below 32768
-constexpr int kNumFastClasses = 4;                 // single-phase tile classes 0..3
-constexpr int kSlowClass = kNumFastClasses;        // 4: generic kernel
-constexpr int kNumSplitClasses = 2;                // 5, 6: two-phase kernels (vtx_sw_split.cuh)
-constexpr int kSplitClass0 = kSlowClass + 1;
-constexpr int kFoldClass = kSplitClass0 + kNumSplitClasses;   // 7: folded kernel (vtx_sw_fold.cuh)
-constexpr int kNumClasses = kFoldClass + 1;
 constexpr int kTileChunk = 8;            // most tiles grabbed per atomic
 
 // fast tile classes: lanes per pair, columns per lane, storage stride (words; CS % 4 == 0, (CS/4) odd
@@ -110,13 +74,14 @@ template <> struct TileClass<2> { static constexpr int LPP = 8, C = 32, CS = 36,
 template <> struct TileClass<3> { static constexpr int LPP = 8, C = 40, CS = 44, THREADS = 384, MINB = 1; };   // n <= 320 per pass
 // Class 3 also takes windows wider than 320 columns (e.g. --padding 200) in several passes of 320 columns: the last
 // column (H + gap, E) of every row is parked in shared memory between passes, like the two-phase kernels do.
-constexpr int kMultiClass = 3;
-constexpr int kMultiMaxRead = 256;       // reads longer than this fall back to the generic kernel for wide windows
-__host__ __device__ constexpr int class_max_n(int cls)
+template <int CLS> constexpr bool tile_class_agrees()
 {
-    return cls == 0 ? 208 : cls == 1 ? 232 : cls == 2 ? 256 : cls == 3 ? 320 : 0x7fffffff;
+    return TileClass<CLS>::LPP * TileClass<CLS>::C == class_max_n(CLS) && 32 / TileClass<CLS>::LPP == int(pairs_per_tile(CLS));
 }
+static_assert(tile_class_agrees<0>() && tile_class_agrees<1>() && tile_class_agrees<2>() && tile_class_agrees<3>(),
+              "vtx_tile_class.cuh: widest window and pairs per tile of the single-phase classes");
 constexpr int kSlowPairsPerWarp = 16;    // generic kernel: one thread per (pair, haplotype)
+static_assert(kSlowPairsPerWarp == int(pairs_per_tile(kSlowClass)), "vtx_tile_class.cuh: pairs per tile of the generic class");
 
 struct SwArgs {
     // staged batch
@@ -136,7 +101,6 @@ struct SwArgs {
     int32_t min_score;              // MIN_SCORE main.rs:30
     int32_t mcap;                   // row-code capacity (even, >= longest read in the batch)
     uint32_t k64k;                  // 65536 as a run-time value (keeps a shift-add on the FMA pipe, see vtx_sw_split.cuh)
-    uint32_t one;                   // 1 as a run-time value (keeps the packed adds on the FMA pipe)
     int32_t multi;                  // class 3 may run several column passes (boundary buffer present in smem)
     // generic kernel only
     uint32_t* scratch;              // [warps][max_hap + 1][32]
@@ -286,7 +250,6 @@ __global__ void __launch_bounds__(TileClass<CLS>::THREADS, TileClass<CLS>::MINB)
             const uint8_t* lane_prof = reinterpret_cast<const uint8_t*>(prof) + g * CS * 4;
             const uint16_t* my_codes = codes + M - g;
             const int steps = mmax + LPP - 1;
-            const uint32_t one = a.one;
             for (int pass = 0; pass < n_pass; ++pass) {
                 if (MULTI && n_pass > 1) { __syncwarp(); build_profile(pass * LPP * C); __syncwarp(); }
                 uint32_t hg[C], f[C];
@@ -321,10 +284,10 @@ __global__ void __launch_bounds__(TileClass<CLS>::THREADS, TileClass<CLS>::MINB)
                             if (c < C) {
                                 const uint32_t fc = __viaddmax_s16x2(f[c], kGE2, hg[c]);     // F[i][c]
                                 e = __viaddmax_s16x2(e, kGE2, eg);                          // E[i][c]
-                                const uint32_t h = sw_h(diag, one, sv[k], fc, e);           // H[i][c]
+                                const uint32_t h = sw_h(diag, sv[k], fc, e);                // H[i][c]
                                 hh[k] = h;
                                 diag = hg[c];
-                                hleft = hadd(h, one, c);                                    // H + goe
+                                hleft = h + kGoeAdd;                                        // H + goe
                                 eg = hleft;
                                 hg[c] = hleft;
                                 f[c] = fc;

@@ -42,12 +42,11 @@
 
 namespace vtx {
 
-constexpr int kFoldP = 96;             // forward-prefix and reversed-suffix columns of the main pass (8 lanes x 12)
-constexpr int kFoldC1 = 12;
+constexpr int kFoldC1 = 12;            // main-pass columns per lane: 8 x 12 = kFoldP
 constexpr int kFoldPPW = 4;            // pairs per warp tile
 constexpr int kFoldR = 19;             // read rows per lane in the middle (8 x 19 = 152)
-constexpr int kFoldMaxRead = 8 * kFoldR;
-constexpr int kFoldMaxMid = 40;        // allele columns: n <= 2 * 96 + 40 = 232
+static_assert(8 * kFoldC1 == kFoldP && 8 * kFoldR == kFoldMaxRead && kFoldPPW == int(pairs_per_tile(kFoldClass)),
+              "vtx_tile_class.cuh: flank columns, longest read and pairs per tile of the folded class");
 // boundary rows kept per read; 156 (not 152) so that the four reads of a tile start 8, 16 and 24 banks apart
 // (152 rows x 8 bytes put reads 0/2 and 1/3 on the same banks: a 2-way conflict on every boundary store and load)
 constexpr int kFoldRows = kFoldMaxRead + 4;
@@ -161,7 +160,6 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
     static_assert(SHARED || S == W, "per-warp tables: one slot per warp");
     const uint32_t run_len = SHARED ? fold_run_len(n_tiles, gridDim.x, W, kTileChunk)
                                     : max(1u, min(uint32_t(kTileChunk), n_tiles / (gridDim.x * W * 16u)));
-    const uint32_t one = a.one;
     uint32_t w_next = 0, w_end = 0, w_locus = 0, w_cached = kFoldNoTile;   // per-warp tables: the warp's chunk
     if (threadIdx.x == 0) ring_init(ring);
     __syncthreads();                                             // the only CTA-wide barrier (see vtx_fold_ring.cuh)
@@ -324,10 +322,10 @@ __global__ void __launch_bounds__(W * 32, 1) vtx_k_sw_fold(const SwArgs a)
                         const int c = 4 * q + k;
                         const uint32_t fc = __viaddmax_s16x2(f[c], kGE2, hg[c]);
                         e = __viaddmax_s16x2(e, kGE2, eg);
-                        const uint32_t h = sw_h(diag, one, sv[k], fc, e);
+                        const uint32_t h = sw_h(diag, sv[k], fc, e);
                         hh[k] = h;
                         diag = hg[c];
-                        hleft = hadd(h, one, c);
+                        hleft = h + kGoeAdd;
                         eg = hleft;
                         hg[c] = hleft;
                         f[c] = fc;

@@ -18,33 +18,22 @@
 
 namespace vtx {
 
-constexpr int kSplitP = 96;            // prefix columns handled by phase 1 (8 lanes x 12)
-constexpr int kSplitC1 = 12;
+constexpr int kSplitC1 = 12;            // phase 1: 8 lanes x 12 columns = kSplitP
 constexpr int kSplitPPW = 8;           // pairs per warp tile
-constexpr int kSplitMaxRead = 256;     // longer reads use the single-phase classes (shared-memory budget)
 
 template <int SCLS> struct SplitClass;
-// COPIES: 2 = the phase-2 profile is stored twice, 16 banks apart, so the two reads of an LDS wavefront never
-// collide; 1 = single copy (2-way conflicts on those loads, 3 KB less shared memory per warp)
-// defaults: one copy and 20 warps/SM for the SNV class (the shared memory of a second copy costs resident warps)
-#ifndef VTX_SPLIT0_COPIES
-#define VTX_SPLIT0_COPIES 1
-#endif
 #ifndef VTX_SPLIT0_THREADS
 #define VTX_SPLIT0_THREADS 320
-#endif
-#ifndef VTX_SPLIT1_COPIES
-#define VTX_SPLIT1_COPIES 1
-#endif
-#ifndef VTX_SPLIT_ONLY
-#define VTX_SPLIT_ONLY 0         // 1 / 2: run only phase 1 / phase 2 (timing experiments; results are wrong)
 #endif
 #ifndef VTX_SPLIT1_THREADS
 #define VTX_SPLIT1_THREADS 256
 #endif
-template <> struct SplitClass<0> { static constexpr int C2 = 27, CS2 = 28, THREADS = VTX_SPLIT0_THREADS, MINB = 2, COPIES = VTX_SPLIT0_COPIES; };   // n <= 96 + 108 = 204 (SNV, pad 100)
-template <> struct SplitClass<1> { static constexpr int C2 = 34, CS2 = 36, THREADS = VTX_SPLIT1_THREADS, MINB = 2, COPIES = VTX_SPLIT1_COPIES; };   // n <= 96 + 136 = 232 (indels <= 30)
-__host__ __device__ constexpr int split_max_n(int scls) { return scls == 0 ? kSplitP + 4 * 27 : kSplitP + 4 * 34; }
+template <> struct SplitClass<0> { static constexpr int C2 = 27, CS2 = 28, THREADS = VTX_SPLIT0_THREADS, MINB = 2; };   // n <= 96 + 108 = 204 (SNV, pad 100)
+template <> struct SplitClass<1> { static constexpr int C2 = 34, CS2 = 36, THREADS = VTX_SPLIT1_THREADS, MINB = 2; };   // n <= 96 + 136 = 232 (indels <= 30)
+static_assert(8 * kSplitC1 == kSplitP && kSplitPPW == int(pairs_per_tile(kSplitClass0)) && kSplitPPW == int(pairs_per_tile(kSplitClass0 + 1)),
+              "vtx_tile_class.cuh: prefix columns and pairs per tile of the two-phase classes");
+static_assert(kSplitP + 4 * SplitClass<0>::C2 == split_max_n(0) && kSplitP + 4 * SplitClass<1>::C2 == split_max_n(1),
+              "vtx_tile_class.cuh: widest window of the two-phase classes");
 
 template <int SCLS>
 __host__ __device__ constexpr size_t split_warp_bytes(int mcap)
@@ -52,7 +41,7 @@ __host__ __device__ constexpr size_t split_warp_bytes(int mcap)
     using SC = SplitClass<SCLS>;
     constexpr int RS2 = (4 * SC::CS2 + 31) / 32 * 32;
     size_t b = size_t(5 * kSplitP) * 4;                         // prof1
-    b += size_t(SC::COPIES * 5 * RS2 + 16) * 4;                  // prof2 (second copy shifted by 16 banks)
+    b += size_t(5 * RS2 + 16) * 4;                               // prof2 and 16 spare words
     b += size_t(4) * (mcap + 8) * 8;                             // boundary column, per unit and row
     b += 16;                                                     // prefix maxima
     b += size_t(kSplitPPW) * (mcap + 16);                        // row codes (u8)
@@ -66,7 +55,6 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
     constexpr int C1 = kSplitC1, C2 = SC::C2, CS2 = SC::CS2, P = kSplitP;
     constexpr int RS1 = P;                                       // 96 words: 3 x 32 banks
     constexpr int RS2 = (4 * CS2 + 31) / 32 * 32;
-    constexpr int COPY2 = SC::COPIES == 2 ? 5 * RS2 + 16 : 0;    // second copy lands 16 banks away
     constexpr int M = 8;
     static_assert(CS2 % 4 == 0 && ((CS2 / 4) & 1) == 1 && CS2 >= C2, "phase-2 stride");
 
@@ -76,7 +64,7 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
     uint8_t* wbase = smem_raw + warp * split_warp_bytes<SCLS>(a.mcap);
     uint32_t* prof1 = reinterpret_cast<uint32_t*>(wbase);
     uint32_t* prof2 = prof1 + 5 * RS1;
-    uint2* bnd = reinterpret_cast<uint2*>(prof2 + SC::COPIES * 5 * RS2 + 16);
+    uint2* bnd = reinterpret_cast<uint2*>(prof2 + 5 * RS2 + 16);
     uint32_t* p1best = reinterpret_cast<uint32_t*>(bnd + 4 * (a.mcap + 8));
     uint8_t* codes = reinterpret_cast<uint8_t*>(p1best + 4);
     const int bnd_stride = a.mcap + 8;
@@ -87,7 +75,6 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
     // small so that every warp still gets >= ~16 grabs (tail balance)
     const uint32_t tile_chunk = max(1u, min(uint32_t(kTileChunk), n_tiles / (gridDim.x * (blockDim.x >> 5) * 16u)));
     const uint32_t k64k = a.k64k;                                // 65536, opaque to ptxas so the merge stays an IMAD
-    const uint32_t one = a.one;                                  // 1, likewise: packed adds as IMAD on the FMA pipe
 
     for (;;) {
         uint32_t chunk = 0;
@@ -124,11 +111,8 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
                         if (j < n_alt) ab = hap_code(__ldg(ah + j));
                     }
 #pragma unroll
-                    for (uint32_t r = 0; r < 5; ++r) {
-                        const uint32_t w = pack2(r == rb ? kProfMatch : kProfMis, r == ab ? kProfMatch : kProfMis);
-                        prof2[r * RS2 + idx] = w;
-                        if (SC::COPIES == 2) prof2[COPY2 + r * RS2 + idx] = w;
-                    }
+                    for (uint32_t r = 0; r < 5; ++r)
+                        prof2[r * RS2 + idx] = pack2(r == rb ? kProfMatch : kProfMis, r == ab ? kProfMatch : kProfMis);
                 }
             }
             // ---- row codes: lane l helps read (l / 4) ----
@@ -168,11 +152,7 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
                 const uint8_t* cB = codes + (2 * u + 1) * code_stride + M - g;
                 const uint32_t* lane_prof = prof1 + g * C1;
                 uint2* my_bnd = bnd + u * bnd_stride;
-#if VTX_SPLIT_ONLY == 2
-                const int steps = 0;                                         // timing experiment: phase 2 alone
-#else
                 const int steps = mmax + 7;
-#endif
                 for (int t = 0; t < steps; ++t) {
                     uint32_t hl = __shfl_up_sync(0xffffffffu, hg_last, 1, 8);
                     uint32_t el = __shfl_up_sync(0xffffffffu, e_last, 1, 8);
@@ -193,10 +173,10 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
                             const int c = 4 * q + k;
                             const uint32_t fc = __viaddmax_s16x2(f[c], kGE2, hg[c]);
                             e = __viaddmax_s16x2(e, kGE2, eg);
-                            const uint32_t h = sw_h(diag, one, sv[k], fc, e);
+                            const uint32_t h = sw_h(diag, sv[k], fc, e);
                             hh[k] = h;
                             diag = hg[c];
-                            hleft = hadd(h, one, c);
+                            hleft = h + kGoeAdd;
                             eg = hleft;
                             hg[c] = hleft;
                             f[c] = fc;
@@ -226,13 +206,9 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
                 uint32_t hg_last = kGOE2, e_last = kNEG2, diag_save = kGOE2;
                 uint32_t best = __byte_perm(p1best[u], 0, sel);              // the prefix maximum counts for ref and alt
                 const uint8_t* cR = codes + r * code_stride + M - g;
-                const uint32_t* lane_prof = prof2 + (w ? COPY2 : 0) + g * CS2;
+                const uint32_t* lane_prof = prof2 + g * CS2;
                 const uint2* my_bnd = bnd + u * bnd_stride;
-#if VTX_SPLIT_ONLY == 1
-                const int steps = 0;                                         // timing experiment: phase 1 alone
-#else
                 const int steps = mmax + 3;
-#endif
                 for (int t = 0; t < steps; ++t) {
                     uint32_t hl = __shfl_up_sync(0xffffffffu, hg_last, 1, 4);
                     uint32_t el = __shfl_up_sync(0xffffffffu, e_last, 1, 4);
@@ -258,10 +234,10 @@ __global__ void __launch_bounds__(SplitClass<SCLS>::THREADS, SplitClass<SCLS>::M
                             if (c < C2) {
                                 const uint32_t fc = __viaddmax_s16x2(f[c], kGE2, hg[c]);
                                 e = __viaddmax_s16x2(e, kGE2, eg);
-                                const uint32_t h = sw_h(diag, one, sv[k], fc, e);
+                                const uint32_t h = sw_h(diag, sv[k], fc, e);
                                 hh[k] = h;
                                 diag = hg[c];
-                                hleft = hadd(h, one, c);
+                                hleft = h + kGoeAdd;
                                 eg = hleft;
                                 hg[c] = hleft;
                                 f[c] = fc;
