@@ -385,6 +385,35 @@ int         vtx_locus_stats_get(vtx_ctx* ctx, const vtx_locus_stats** out, uint6
 int         vtx_set_donors(vtx_ctx* ctx, uint32_t n_donors, uint64_t n_rows, const uint8_t* dosage, double error_rate);
 int         vtx_donor_ll_get(vtx_ctx* ctx, const int64_t** ll, const uint64_t** counts, uint32_t* n_cols, uint32_t* n_hyp);
 
+/* ---- genotype-free clustering of pooled cells (the CLI's --out-clusters; DESIGN.md §5g) ------------------------------------
+ * An allele-fraction EM with k clusters over host count entries (row, col, ref_cnt, alt_cnt), e.g. a finished vtx_result:
+ * strictly ascending (row, col) in row-major order, row < n_rows, col < n_cols.  Entries with ref + alt = 0 are ignored.  A row
+ * is used when at least 4 cells have ref > 0 there and at least 4 have alt > 0.  Cluster k has theta_kv =
+ * (A_kv + 2^16) / (T_kv + 2^17) at row v, A / T the cells' ALT / REF + ALT counts weighted by W_ck <= 2^16.  `restarts` EMs
+ * start from seeded random thetas and run until W repeats or for 200 iterations; the one with the largest
+ * sum_c max_k LL_ck wins (ties: the lowest restart).  Its clusters are ordered by sum_c W_ck, descending (ties: EM index).
+ * Everything is integer or correctly rounded double arithmetic: the result is a function of the entries and the parameters.
+ *
+ * out->ll[c * n_hyp + h] (int64, x VTX_DONOR_LL_SCALE) scores the cell over used rows against the n_hyp = k + k(k-1)/2
+ * hypotheses in vtx_set_donors' order (singlet C_h, then the 50/50 doublets); counts[c * 3 + {0, 1, 2}] = used entries, REF, ALT.
+ * alt_w / depth_w [row * k + j] are the winner's final A, T over every row (x 2^16); restart_score / restart_iters per restart.
+ * Library-owned host memory, valid until the next vtx_cluster_cells or vtx_destroy.  VTX_E_STATE while submits are unfinished
+ * (between a submit and its finish); VTX_E_INVALID for k outside 2..32, restarts outside 1..64, a bad entry, or a row whose
+ * ref + alt molecules times 2^16 (plus 2^17) reach 2^53; VTX_E_NOMEM when the device cannot hold 28 bytes per entry,
+ * restarts x n_cols x k x 4 bytes of weights and restarts x n_rows x k x 8 bytes of tables. */
+typedef struct vtx_cluster_params { uint32_t k, restarts; uint64_t seed; } vtx_cluster_params;
+typedef struct vtx_clusters {
+    uint32_t k, n_cols, n_hyp, best_restart; uint64_t n_rows, rows_used;
+    const int64_t* ll;            /* [n_cols][n_hyp] x 2^24, canonical cluster order */
+    const uint64_t* counts;       /* [n_cols][3] variants, ref, alt over used rows */
+    const uint8_t* row_used;      /* [n_rows] */
+    const int64_t* alt_w; const int64_t* depth_w;   /* [n_rows][k] x 2^16: final A, T over all rows */
+    const int64_t* restart_score; const uint32_t* restart_iters;   /* [restarts] */
+} vtx_clusters;
+int         vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                              const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params,
+                              vtx_clusters* out);
+
 /* Injective code of a cell-barcode tag of the form [ACGT]{1,24}(-N)? with N = 1..99 written without a leading zero:
  * 2 bits per base, 5 bits length, 7 bits N (0 = no suffix); < 2^60.  Returns VTX_NO_CB_KEY if the bytes have another
  * form -- the caller then lists them as an exotic tag (VTX_CB_EXOTIC | i). */

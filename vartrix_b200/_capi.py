@@ -32,7 +32,7 @@ SYMBOLS = [
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
     "vtx_set_min_base_quality", "vtx_bam_low_base_quality", "vtx_set_locus_stats", "vtx_locus_stats_get",
-    "vtx_set_donors", "vtx_donor_ll_get",
+    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
 CB_EXOTIC = 0x8000000000000000
@@ -105,6 +105,17 @@ LOCUS_STATS_FIELDS = ("row", "fetched", "low_mapq", "non_primary", "duplicate", 
 
 class LocusStats(C.Structure):     # vtx_locus_stats
     _fields_ = [(f, C.c_uint32) for f in LOCUS_STATS_FIELDS]
+
+
+class ClusterParams(C.Structure):  # vtx_cluster_params
+    _fields_ = [("k", C.c_uint32), ("restarts", C.c_uint32), ("seed", C.c_uint64)]
+
+
+class Clusters(C.Structure):       # vtx_clusters
+    _fields_ = [("k", C.c_uint32), ("n_cols", C.c_uint32), ("n_hyp", C.c_uint32), ("best_restart", C.c_uint32),
+                ("n_rows", C.c_uint64), ("rows_used", C.c_uint64), ("ll", C.POINTER(C.c_int64)), ("counts", C.POINTER(C.c_uint64)),
+                ("row_used", C.POINTER(C.c_uint8)), ("alt_w", C.POINTER(C.c_int64)), ("depth_w", C.POINTER(C.c_int64)),
+                ("restart_score", C.POINTER(C.c_int64)), ("restart_iters", C.POINTER(C.c_uint32))]
 
 
 class Metrics(C.Structure):
@@ -190,6 +201,9 @@ def load():
     L.vtx_donor_ll_get.restype = C.c_int
     L.vtx_donor_ll_get.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int64)), C.POINTER(C.POINTER(C.c_uint64)),
                                    C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+    L.vtx_cluster_cells.restype = C.c_int
+    L.vtx_cluster_cells.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                    C.POINTER(ClusterParams), C.POINTER(Clusters)]
     L.vtx_pack_cb.restype = C.c_uint64
     L.vtx_pack_cb.argtypes = [C.c_char_p, C.c_uint32]
     L.vtx_gather_start.restype = C.c_int

@@ -4,6 +4,8 @@
 // Matrix-Market / label files.  `--dump-staged` stops after staging (no GPU needed; used by the tests).
 #include <atomic>
 #include <condition_variable>
+#include <cctype>
+#include <cerrno>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -23,6 +25,7 @@
 
 #include "stager.hpp"
 #include "../vtx_donors.cuh"
+#include "../vtx_clusters.cuh"
 
 using namespace vtxhost;
 
@@ -53,6 +56,10 @@ struct Opts {
     std::string out_donors, donors;            // --out-donors FILE, --donors NAME,NAME,...
     double donor_error_rate = 0.01;            // --donor-error-rate
     bool donor_error_rate_given = false;
+    std::string out_clusters, out_cluster_alleles;     // --out-clusters FILE, --out-cluster-alleles FILE
+    uint32_t clusters = 0, cluster_restarts = 8;       // --clusters K, --cluster-restarts R
+    uint64_t cluster_seed = 0;                         // --cluster-seed S
+    bool cluster_restarts_given = false, cluster_seed_given = false;
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
     uint32_t min_base_quality = 0;     // --min-base-quality (0: off)
@@ -77,6 +84,12 @@ void usage()
          "                              doublet log-likelihoods from the cell's REF / ALT counts, the best pair and the call\n"
          "      --donors LIST           The VCF samples that are the pool's donors, e.g. S1,S4,S2 (2 to 32) [every sample]\n"
          "      --donor-error-rate E    Per-molecule error rate of the donor model, 1e-6 .. 0.25 [0.01]\n"
+         "      --out-clusters FILE     Cluster the cells into --clusters donors without genotypes (TSV, one line per barcode, the\n"
+         "                              --out-donors columns with clusters C0, C1, ... for donors): allele-fraction EM, doublet calls\n"
+         "      --clusters K            Number of clusters, 2 .. 32 (needed by --out-clusters)\n"
+         "      --cluster-restarts R    EM restarts from random starts, the best one is kept, 1 .. 64 [8]\n"
+         "      --cluster-seed S        Seed of the restarts' random starts, 0 .. 2^64-1 [0]\n"
+         "      --out-cluster-alleles FILE  Per-variant REF / ALT counts of every cluster (TSV, one line per VCF record)\n"
          "  -p, --padding INT           Padding on both sides of the variant [100]\n"
          "  -s, --scoring-method M      consensus | coverage | alt_frac [consensus]\n"
          "      --ref-matrix FILE       Reference matrix (coverage mode) [ref_matrix.mtx]\n"
@@ -155,6 +168,23 @@ bool parse(int argc, char** argv, Opts* o)
             o->donor_error_rate = x;
             o->donor_error_rate_given = true;
         }
+        else if (a == "--out-clusters") o->out_clusters = v();
+        else if (a == "--out-cluster-alleles") o->out_cluster_alleles = v();
+        else if (a == "--clusters" || a == "--cluster-restarts" || a == "--cluster-seed") {
+            const std::string t = v();
+            char* end = nullptr;
+            errno = 0;
+            const unsigned long long x = strtoull(t.c_str(), &end, 10);
+            const bool is_k = a == "--clusters", is_r = a == "--cluster-restarts";
+            const unsigned long long lo = is_k ? vtx::clusters::kMinK : is_r ? 1 : 0, hi = is_k ? vtx::clusters::kMaxK : is_r ? vtx::clusters::kMaxRestarts : ~0ull;
+            if (t.empty() || !isdigit((unsigned char)t[0]) || *end != 0 || errno == ERANGE || x < lo || x > hi) {
+                fprintf(stderr, "error: %s must be an integer from %llu to %llu, not '%s'\n", a.c_str(), lo, hi, t.c_str());
+                return false;
+            }
+            if (is_k) o->clusters = uint32_t(x);
+            else if (is_r) { o->cluster_restarts = uint32_t(x); o->cluster_restarts_given = true; }
+            else { o->cluster_seed = x; o->cluster_seed_given = true; }
+        }
         else if (a == "-p" || a == "--padding") o->padding = atol(v().c_str());
         else if (a == "-s" || a == "--scoring-method") o->scoring = v();
         else if (a == "--ref-matrix") { o->ref_matrix = v(); o->ref_matrix_given = true; }
@@ -208,6 +238,18 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --donors and --donor-error-rate only apply with --out-donors\n");
         return false;
     }
+    if (o->out_clusters.empty() != (o->clusters == 0)) {
+        fprintf(stderr, "error: --out-clusters and --clusters need each other\n");
+        return false;
+    }
+    if (o->out_clusters.empty() && (o->cluster_restarts_given || o->cluster_seed_given || !o->out_cluster_alleles.empty())) {
+        fprintf(stderr, "error: --cluster-restarts, --cluster-seed and --out-cluster-alleles only apply with --out-clusters\n");
+        return false;
+    }
+    if (!o->out_clusters.empty() && !o->dump_staged.empty()) {
+        fprintf(stderr, "error: --out-clusters clusters what the GPU run counts: it cannot be combined with --dump-staged\n");
+        return false;
+    }
     if (o->threads < 1) o->threads = 1;
     if (o->shard_loci < 0) o->shard_loci = 0;
     if (o->devices.empty()) o->devices.push_back(int(o->device));
@@ -230,6 +272,8 @@ void check_inputs_exist(const Opts& o)
     if (o.dump_staged.empty()) { validate_output_path(o.out_matrix); validate_output_path(o.ref_matrix); }
     if (!o.out_variant_stats.empty()) validate_output_path(o.out_variant_stats);
     if (!o.out_donors.empty()) validate_output_path(o.out_donors);
+    if (!o.out_clusters.empty()) validate_output_path(o.out_clusters);
+    if (!o.out_cluster_alleles.empty()) validate_output_path(o.out_cluster_alleles);
     if (!exists(o.fasta + ".fai")) { LOG_ERR("File %s.fai does not exist", o.fasta.c_str()); exit(1); }
     const size_t dot = o.bam.find_last_of('.');
     const std::string ext = dot == std::string::npos ? "" : o.bam.substr(dot + 1);
@@ -452,6 +496,26 @@ bool write_donors(const std::string& path, const std::vector<std::string>& barco
     return fclose(f) == 0;
 }
 
+// --out-cluster-alleles: one line per VCF record in row order, the cluster's REF and ALT molecules (x 2^16 sums scaled back)
+bool write_cluster_alleles(const std::string& path, const std::vector<VcfRecord>& recs, const vtx_clusters& cl)
+{
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    fputs("variant\tused", f);
+    for (uint32_t j = 0; j < cl.k; ++j) fprintf(f, "\tref_C%u\talt_C%u", j, j);
+    fputc('\n', f);
+    const double w = double(vtx::clusters::kW);
+    for (size_t v = 0; v < recs.size(); ++v) {
+        fprintf(f, "%s_%lld\t%u", recs[v].chrom.c_str(), (long long)recs[v].pos0, unsigned(cl.row_used[v]));
+        for (uint32_t j = 0; j < cl.k; ++j) {
+            const int64_t a = cl.alt_w[v * cl.k + j], t = cl.depth_w[v * cl.k + j];
+            fprintf(f, "\t%.4f\t%.4f", double(t - a) / w, double(a) / w);
+        }
+        fputc('\n', f);
+    }
+    return fclose(f) == 0;
+}
+
 }  // namespace
 
 // One GPU of the run: its own engine context, a contiguous range of shards, a thread that feeds it in order.
@@ -524,7 +588,8 @@ int main(int argc, char** argv)
                 vtx_config cfg{};
                 cfg.device = cuda_index[d];
                 cfg.mode = o.scoring == "consensus" ? VTX_MODE_CONSENSUS : o.scoring == "coverage" ? VTX_MODE_COVERAGE : VTX_MODE_ALT_FRAC;
-                cfg.flags = VTX_F_VALUES_ONLY;       // the writers need row, col and the matrix values only
+                // the matrix writers need row, col and the values only; --out-clusters also needs the REF / ALT counts
+                cfg.flags = o.out_clusters.empty() ? VTX_F_VALUES_ONLY : 0u;
                 if (o.collapse_mates) cfg.flags |= VTX_F_NAME_KEYS;      // name keys through the UMI collapse
                 cfg.use_umi = o.umi || o.collapse_mates; cfg.match = 1; cfg.mismatch = -5; cfg.gap_open = -5; cfg.gap_extend = -1; cfg.min_score = 25;
                 cfg.band_k = 6; cfg.band_w = 20; cfg.band_mode = VTX_BAND_FULL;          // main.rs:33-34
@@ -916,6 +981,26 @@ int main(int argc, char** argv)
         LOG_INFO("Donors: %zu (%s), error rate %g; rows with a genotype for every donor: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
                  donors.names.size(), list.c_str(), o.donor_error_rate, (unsigned long long)donors.usable, recs.size(),
                  (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
+    }
+    if (!o.out_clusters.empty()) {      // once, on lane 0, over every lane's triplets
+        validate_output_path(o.out_clusters);
+        if (!o.out_cluster_alleles.empty()) validate_output_path(o.out_cluster_alleles);
+        const vtx_cluster_params cp{ o.clusters, o.cluster_restarts, o.cluster_seed };
+        vtx_clusters cl{};
+        if (vtx_cluster_cells(ctx, res.n, res.row, res.col, res.ref_cnt, res.alt_cnt, recs.size(), uint32_t(bcs.keys.size()), &cp, &cl) != VTX_OK) {
+            printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx)); rc = 1;
+        } else {
+            std::vector<std::string> names;
+            for (uint32_t j = 0; j < cl.k; ++j) names.push_back("C" + std::to_string(j));
+            const std::vector<int64_t> ll(cl.ll, cl.ll + size_t(cl.n_cols) * cl.n_hyp);
+            const std::vector<uint64_t> cnt(cl.counts, cl.counts + size_t(cl.n_cols) * 3);
+            uint64_t calls[3] = { 0, 0, 0 };
+            if (!write_donors(o.out_clusters, bcs.keys, names, ll, cnt, calls)) { LOG_ERR("error writing cluster file"); rc = 1; }
+            if (!o.out_cluster_alleles.empty() && !write_cluster_alleles(o.out_cluster_alleles, recs, cl)) { LOG_ERR("error writing cluster allele file"); rc = 1; }
+            LOG_INFO("Clusters: %u, restarts %u, seed %llu; best restart %u after %u iterations; rows used: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
+                     cl.k, o.cluster_restarts, (unsigned long long)o.cluster_seed, cl.best_restart, cl.restart_iters[cl.best_restart],
+                     (unsigned long long)cl.rows_used, recs.size(), (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
+        }
     }
     LOG_INFO("[%.3f s] outputs written", now_s());
     double sum = 0;

@@ -8,6 +8,7 @@
 #include "vtx_stage.cuh"
 #include "vtx_locus_stats.cuh"
 #include "vtx_donors.cuh"
+#include "vtx_clusters.cuh"
 
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
@@ -148,7 +149,14 @@ struct vtx_ctx {
     HostBuf h_donor;
     size_t h_donor_cap = 0;                             // bytes
     bool donor_valid = false;                           // h_donor holds the last finished result set
-    HostBuf h_stage;                                    // scalars read back between the staging phases
+    // vtx_cluster_cells: device work buffers and the host outputs of the last call
+    DBuf cl_row, cl_col, cl_r, cl_a, cl_used, cl_used_rows, cl_row_start, cl_cell_count, cl_cell_start, cl_c_row, cl_c_r, cl_c_a,
+        cl_la, cl_lr, cl_w, cl_flags, cl_A, cl_T, cl_ll, cl_cnt;
+    std::vector<int64_t> h_cl_ll, h_cl_A, h_cl_T, h_cl_score;
+    std::vector<uint64_t> h_cl_cnt;
+    std::vector<uint8_t> h_cl_used;
+    std::vector<uint32_t> h_cl_iters;
+    HostBuf h_stage;                                   // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
 
@@ -1544,6 +1552,211 @@ int vtx_donor_ll_get(vtx_ctx* ctx, const int64_t** ll, const uint64_t** counts, 
     *counts = reinterpret_cast<const uint64_t*>(*ll + size_t(ctx->donor_last_cols) * H);
     *n_cols = ctx->donor_last_cols;
     *n_hyp = H;
+    return VTX_OK;
+}
+
+int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                      const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params, vtx_clusters* out)
+{
+    using namespace clusters;
+    if (!ctx || !params || !out) return VTX_E_INVALID;
+    *out = vtx_clusters{};
+    if (!ctx->finished || ctx->gather_pending)
+        return set_err(ctx, VTX_E_STATE, "vtx_cluster_cells: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const uint32_t K = params->k, R = params->restarts;
+    if (K < kMinK || K > kMaxK) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: k = %u; 2 to 32 clusters are supported", K);
+    if (R < 1 || R > kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: %u restarts; 1 to 64 are supported", R);
+    if (n && (!row || !col || !ref_cnt || !alt_cnt)) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: an entry array is NULL");
+    if (n > 0xFFFFFFFFull || n_rows > 0xFFFFFFFFull)
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: %llu entries over %llu rows; both must be below 2^32",
+                       (unsigned long long)n, (unsigned long long)n_rows);
+    const uint32_t H = donors::n_hyp(K);
+    // device memory, before any host table of n_rows entries: the by-row entries (16 B) and their by-cell copy (12 B), the
+    // weights, the tables, the final sums and the outputs
+    const double need = double(n) * 28 + double(n_rows) * (5 + 16.0 * K) + double(n_cols) * (12 + 24 + 8.0 * H) +
+                        double(R) * n_cols * K * 4 + double(R) * double(n_rows) * K * 8;
+    {
+        CK(cudaSetDevice(ctx->device));
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        size_t held = 0;
+        for (DBuf* b : { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_used_rows, &ctx->cl_row_start,
+                         &ctx->cl_cell_count, &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_la, &ctx->cl_lr,
+                         &ctx->cl_w, &ctx->cl_flags, &ctx->cl_A, &ctx->cl_T, &ctx->cl_ll, &ctx->cl_cnt })
+            held += b->cap;
+        if (need > double(free_b) + double(held))
+            return set_err(ctx, VTX_E_NOMEM, "vtx_cluster_cells needs %.0f MB of device memory, %.0f MB are free", need * 1e-6,
+                           (double(free_b) + double(held)) * 1e-6);
+    }
+    // validate the entries in one pass; rows are contiguous, so the per-row counts need no table
+    std::vector<uint32_t> row_start(size_t(n_rows) + 1, 0);
+    ctx->h_cl_used.assign(size_t(n_rows), 0);
+    std::vector<uint32_t> used_rows;
+    const uint64_t kMaxMolecules = ((1ull << 53) - (1ull << 17)) >> 16;     // molecules x 2^16 + 2^17 stays below 2^53
+    for (uint64_t i = 0; i < n;) {
+        const uint32_t v = row[i];
+        if (v >= n_rows) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu has row %u >= n_rows %llu", (unsigned long long)i, v, (unsigned long long)n_rows);
+        if (i && v < row[i - 1]) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu: rows are not ascending", (unsigned long long)i);
+        uint32_t with_ref = 0, with_alt = 0;
+        uint64_t molecules = 0;
+        const uint64_t i0 = i;
+        for (; i < n && row[i] == v; ++i) {
+            if (col[i] >= n_cols) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu has col %u >= n_cols %u", (unsigned long long)i, col[i], n_cols);
+            if (i > i0 && col[i] <= col[i - 1])
+                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu: (row, col) is not strictly ascending", (unsigned long long)i);
+            with_ref += ref_cnt[i] > 0;
+            with_alt += alt_cnt[i] > 0;
+            molecules += uint64_t(ref_cnt[i]) + alt_cnt[i];
+            if (molecules > kMaxMolecules)
+                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: row %u holds more than %llu molecules; its weighted sums would not be exact", v,
+                               (unsigned long long)kMaxMolecules);
+        }
+        row_start[size_t(v) + 1] = uint32_t(i - i0);
+        if (with_ref >= kMinCells && with_alt >= kMinCells) { ctx->h_cl_used[v] = 1; used_rows.push_back(v); }
+    }
+    for (uint64_t v = 0; v < n_rows; ++v) row_start[v + 1] += row_start[v];
+
+    cudaStream_t st = ctx->stream;
+    const size_t nb = size_t(n) * 4 + 4;
+    ENS(ctx->cl_row, nb); ENS(ctx->cl_col, nb); ENS(ctx->cl_r, nb); ENS(ctx->cl_a, nb);
+    ENS(ctx->cl_c_row, nb); ENS(ctx->cl_c_r, nb); ENS(ctx->cl_c_a, nb);
+    ENS(ctx->cl_used, size_t(n_rows) + 1);
+    ENS(ctx->cl_used_rows, used_rows.size() * 4 + 4);
+    ENS(ctx->cl_row_start, row_start.size() * 4);
+    ENS(ctx->cl_cell_count, (size_t(n_cols) + 1) * 4);
+    ENS(ctx->cl_cell_start, (size_t(n_cols) + 1) * 4);
+    const size_t tab = size_t(R) * size_t(n_rows) * K * 4 + 4;
+    ENS(ctx->cl_la, tab); ENS(ctx->cl_lr, tab);
+    ENS(ctx->cl_w, size_t(R) * n_cols * K * 4 + 4);
+    const size_t flag_bytes = size_t(R + (R & 1)) * 4 + size_t(R) * 8;     // R changed flags, then R scores (8-aligned)
+    ENS(ctx->cl_flags, flag_bytes);
+    ENS(ctx->cl_A, size_t(n_rows) * K * 8 + 8); ENS(ctx->cl_T, size_t(n_rows) * K * 8 + 8);
+    ENS(ctx->cl_ll, size_t(n_cols) * H * 8 + 8); ENS(ctx->cl_cnt, size_t(n_cols) * 24 + 8);
+    if (n) {
+        CK(cudaMemcpyAsync(ctx->cl_row.p, row, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_r.p, ref_cnt, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_a.p, alt_cnt, n * 4, cudaMemcpyHostToDevice, st));
+    }
+    if (n_rows) CK(cudaMemcpyAsync(ctx->cl_used.p, ctx->h_cl_used.data(), n_rows, cudaMemcpyHostToDevice, st));
+    if (!used_rows.empty()) CK(cudaMemcpyAsync(ctx->cl_used_rows.p, used_rows.data(), used_rows.size() * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->cl_row_start.p, row_start.data(), row_start.size() * 4, cudaMemcpyHostToDevice, st));
+
+    // the by-cell index of the used entries
+    const uint32_t nn = uint32_t(n);
+    const unsigned egrid = std::max(1u, std::min(blocks_for(n, kClThreads), unsigned(ctx->n_sm) * 16));
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    vtx_k_cl_count<<<egrid, kClThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                  P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_count));
+    CK(cudaGetLastError());
+    int rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->cl_cell_count), n_cols, P<uint32_t>(ctx->cl_cell_start), nullptr);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    vtx_k_cl_scatter<<<egrid, kClThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                    P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_start),
+                                                    P<uint32_t>(ctx->cl_cell_count), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r),
+                                                    P<uint32_t>(ctx->cl_c_a));
+    CK(cudaGetLastError());
+    const CellEntries ce{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
+
+    // the EM: every active restart in the same launches; the host reads the restarts' flags and scores once per iteration
+    const uint32_t n_used = uint32_t(used_rows.size());
+    if (n_used) {
+        const unsigned igrid = std::max(1u, std::min(blocks_for(uint64_t(R) * n_used * K, kClThreads), unsigned(ctx->n_sm) * 16));
+        vtx_k_cl_init<<<igrid, kClThreads, 0, st>>>(params->seed, R, K, n_used, P<uint32_t>(ctx->cl_used_rows), n_rows,
+                                                     P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr));
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemsetAsync(ctx->cl_w.p, 0xFF, size_t(R) * n_cols * K * 4, st));         // no weight is 2^32 - 1: the first E-step changes W
+    ctx->h_cl_score.assign(R, 0);
+    ctx->h_cl_iters.assign(R, 0);
+    Active act{};
+    for (uint32_t s = 0; s < R; ++s) act.s[act.n++] = uint8_t(s);
+    uint32_t* d_changed = P<uint32_t>(ctx->cl_flags);
+    unsigned long long* d_score = reinterpret_cast<unsigned long long*>(d_changed + R + (R & 1));
+    std::vector<uint32_t> h_flags(flag_bytes / 4);
+    for (uint32_t it = 1; act.n; ++it) {
+        CK(cudaMemsetAsync(ctx->cl_flags.p, 0, flag_bytes, st));
+        if (n_cols) {
+            const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(act.n) * n_cols * 32, kClThreads), unsigned(ctx->n_sm) * 16));
+            vtx_k_cl_estep<<<g, kClThreads, 0, st>>>(act, ce, n_cols, n_rows, K, P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr),
+                                                     P<uint32_t>(ctx->cl_w), d_changed, d_score);
+            CK(cudaGetLastError());
+        }
+        CK(cudaMemcpyAsync(h_flags.data(), ctx->cl_flags.p, flag_bytes, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        const uint64_t* h_score = reinterpret_cast<const uint64_t*>(h_flags.data() + R + (R & 1));
+        Active next{};
+        for (uint32_t i = 0; i < act.n; ++i) {
+            const uint32_t s = act.s[i];
+            ctx->h_cl_iters[s] = it;
+            ctx->h_cl_score[s] = int64_t(h_score[s]);
+            if (h_flags[s] && it < kMaxIters) next.s[next.n++] = uint8_t(s);
+        }
+        act = next;
+        if (act.n && n_used) {
+            const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(act.n) * n_used * 32, kClThreads), unsigned(ctx->n_sm) * 16));
+            vtx_k_cl_mstep<<<g, kClThreads, 0, st>>>(act, n_used, P<uint32_t>(ctx->cl_used_rows), P<uint32_t>(ctx->cl_row_start),
+                                                     P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a),
+                                                     P<uint32_t>(ctx->cl_w), n_cols, n_rows, K, P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr));
+            CK(cudaGetLastError());
+        }
+    }
+    uint32_t best = 0;
+    for (uint32_t s = 1; s < R; ++s)
+        if (ctx->h_cl_score[s] > ctx->h_cl_score[best]) best = s;
+
+    // canonical order: the best restart's clusters by sum_c W_ck, descending, ties by EM index
+    std::vector<uint32_t> w_best(size_t(n_cols) * K);
+    if (n_cols) CK(cudaMemcpy(w_best.data(), P<uint32_t>(ctx->cl_w) + size_t(best) * n_cols * K, w_best.size() * 4, cudaMemcpyDeviceToHost));
+    std::vector<uint64_t> tot(K, 0);
+    for (size_t i = 0; i < w_best.size(); ++i) tot[i % K] += w_best[i];
+    std::vector<uint32_t> order(K);
+    for (uint32_t k = 0; k < K; ++k) order[k] = k;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return tot[x] > tot[y]; });
+    Perm perm{};
+    for (uint32_t j = 0; j < K; ++j) perm.k[j] = uint8_t(order[j]);
+
+    // the final M-step over every row, then the scoring
+    if (n_rows) {
+        const unsigned g = std::max(1u, std::min(blocks_for(n_rows * 32, kClThreads), unsigned(ctx->n_sm) * 16));
+        vtx_k_cl_final<<<g, kClThreads, 0, st>>>(perm, n_rows, P<uint32_t>(ctx->cl_row_start), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                 P<uint32_t>(ctx->cl_a), P<uint32_t>(ctx->cl_w) + size_t(best) * n_cols * K, K,
+                                                 P<int64_t>(ctx->cl_A), P<int64_t>(ctx->cl_T));
+        CK(cudaGetLastError());
+    }
+    if (n_cols) {
+        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_cols) * 32, kClThreads), unsigned(ctx->n_sm) * 8));
+        const int64_t* A = P<int64_t>(ctx->cl_A);
+        const int64_t* T = P<int64_t>(ctx->cl_T);
+        int64_t* ll = P<int64_t>(ctx->cl_ll);
+        uint64_t* cnt = P<uint64_t>(ctx->cl_cnt);
+        if (H <= 32) vtx_k_cl_score<1><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
+        else if (H <= 64) vtx_k_cl_score<2><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
+        else if (H <= 160) vtx_k_cl_score<5><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
+        else if (H <= 288) vtx_k_cl_score<9><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
+        else vtx_k_cl_score<17><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
+        CK(cudaGetLastError());
+    }
+    ctx->h_cl_ll.resize(size_t(n_cols) * H);
+    ctx->h_cl_cnt.resize(size_t(n_cols) * 3);
+    ctx->h_cl_A.resize(size_t(n_rows) * K);
+    ctx->h_cl_T.resize(size_t(n_rows) * K);
+    if (n_cols) {
+        CK(cudaMemcpyAsync(ctx->h_cl_ll.data(), ctx->cl_ll.p, ctx->h_cl_ll.size() * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_cl_cnt.data(), ctx->cl_cnt.p, ctx->h_cl_cnt.size() * 8, cudaMemcpyDeviceToHost, st));
+    }
+    if (n_rows) {
+        CK(cudaMemcpyAsync(ctx->h_cl_A.data(), ctx->cl_A.p, ctx->h_cl_A.size() * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_cl_T.data(), ctx->cl_T.p, ctx->h_cl_T.size() * 8, cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+
+    out->k = K; out->n_cols = n_cols; out->n_hyp = H; out->best_restart = best;
+    out->n_rows = n_rows; out->rows_used = n_used;
+    out->ll = ctx->h_cl_ll.data(); out->counts = ctx->h_cl_cnt.data(); out->row_used = ctx->h_cl_used.data();
+    out->alt_w = ctx->h_cl_A.data(); out->depth_w = ctx->h_cl_T.data();
+    out->restart_score = ctx->h_cl_score.data(); out->restart_iters = ctx->h_cl_iters.data();
     return VTX_OK;
 }
 

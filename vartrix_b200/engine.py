@@ -612,6 +612,33 @@ class Engine:
         return (np.ctypeslib.as_array(ll, shape=(nc * nh,)).reshape(nc, nh).copy(),
                 np.ctypeslib.as_array(cnt, shape=(nc * 3,)).reshape(nc, 3).copy())
 
+    def cluster_cells(self, row, col, ref, alt, n_rows: int, n_cols: int, k: int, restarts: int = 8, seed: int = 0) -> dict:
+        """Genotype-free clustering of the cells (vtx_cluster_cells, include/vartrix_b200.h; DESIGN.md §5g): count entries
+        (row, col, REF, ALT) strictly ascending by (row, col), e.g. a finished coverage result's row / col / ref_cnt / alt_cnt.
+        -> dict of NumPy copies: ll int64[n_cols, H] (x 2^24), counts uint64[n_cols, 3], row_used uint8[n_rows],
+        alt_w / depth_w int64[n_rows, k] (x 2^16), restart_score int64[restarts], restart_iters uint32[restarts], and the
+        scalars k, n_hyp, best_restart, rows_used."""
+        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
+        n = len(arrs[0])
+        if any(len(x) != n for x in arrs):
+            raise ValueError("row, col, ref and alt must have the same length")
+        out = _capi.Clusters()
+        p = _capi.ClusterParams(int(k), int(restarts), int(seed) & 0xFFFFFFFFFFFFFFFF)
+        ptr = [x.ctypes.data if n else None for x in arrs]
+        self._ck(self._L.vtx_cluster_cells(self._h, n, *ptr, int(n_rows), int(n_cols), C.byref(p), C.byref(out)), "vtx_cluster_cells")
+
+        def arr(ptr, count, dtype, shape):
+            if count == 0:
+                return np.zeros(shape, dtype)
+            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
+        nc, nh, nr, kk = int(out.n_cols), int(out.n_hyp), int(out.n_rows), int(out.k)
+        return dict(k=kk, n_hyp=nh, best_restart=int(out.best_restart), rows_used=int(out.rows_used),
+                    ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
+                    row_used=arr(out.row_used, nr, np.uint8, (nr,)), alt_w=arr(out.alt_w, nr * kk, np.int64, (nr, kk)),
+                    depth_w=arr(out.depth_w, nr * kk, np.int64, (nr, kk)),
+                    restart_score=arr(out.restart_score, int(restarts), np.int64, (int(restarts),)),
+                    restart_iters=arr(out.restart_iters, int(restarts), np.uint32, (int(restarts),)))
+
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()
 
