@@ -414,6 +414,39 @@ int         vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, con
                               const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params,
                               vtx_clusters* out);
 
+/* ---- donor assignment against ambient RNA (the CLI's --ambient-rna; DESIGN.md §5h) -----------------------------------------
+ * vtx_set_donors' model over host count entries (row, col, ref_cnt, alt_cnt) as vtx_cluster_cells takes them, with the pool's
+ * ALT fraction mixed into every hypothesis: at row v, q_vs = (1 - rho) q_s + rho f_v and 1 - q_vs = (1 - rho)(1 - q_s) +
+ * rho (1 - f_v), f_v = (A_v + 1) / (T_v + 2) and 1 - f_v = (T_v - A_v + 1) / (T_v + 2) with A_v / T_v the sums of alt / ref + alt
+ * over every entry at row v, rho = m / 1000 for m in 0..500.  The constants are llrint(log(q) 2^24) with vtx_cluster_cells'
+ * correctly rounded log, so at rho = 0 they equal vtx_set_donors' wherever the two logs round alike.  dosage[row * n_donors + d]
+ * as vtx_set_donors takes it, for every row < n_rows; a row is usable when every donor has a dosage there.
+ * rho_permille = m fixes rho; -1 estimates it: J(m) = sum over cells with variants of max_h LL_ch is evaluated at m = 0, 10, ...,
+ * 500 and then at every m within 9 of the best of those; the largest J wins (ties: the smallest m).  The cells are then scored
+ * at the winner.  grid_batch > 0 caps the m values scored per pass (0: as device memory allows); it does not change the result.
+ *
+ * out->ll [c * n_hyp + h] (x VTX_DONOR_LL_SCALE) and counts [c * 3 + {0, 1, 2}] as vtx_donor_ll_get returns them, at the chosen
+ * m (out->rho_permille).  grid_permille / grid_objective / grid_calls [i * 3 + {singlet, doublet, unassigned}] per evaluated m,
+ * ascending (the calls use vtx_set_donors' rule with T = 5 nats); row_alt / row_depth [row] = A_v, T_v.  Library-owned host
+ * memory, valid until the next vtx_donors_ambient or vtx_destroy.  VTX_E_STATE while submits are unfinished; VTX_E_INVALID for
+ * n_donors outside 2..32, error_rate outside [1e-6, 0.25], rho_permille outside -1..500, a dosage other than 0, 1, 2 or
+ * VTX_GT_MISSING, a bad entry (as vtx_cluster_cells), or a row whose T_v + 2 reaches 2^53; VTX_E_NOMEM when the device cannot
+ * hold the entries (28 bytes each), 21 bytes per row, the cells' log-likelihoods and one m's tables (40 bytes per usable row that
+ * an entry touches). */
+typedef struct vtx_ambient_params {
+    uint32_t n_donors; double error_rate; int32_t rho_permille;      /* -1: estimate */
+    uint32_t grid_batch;                                              /* 0: as memory allows; else at most this many m per pass */
+} vtx_ambient_params;
+typedef struct vtx_ambient {
+    uint32_t n_donors, n_cols, n_hyp, rho_permille, n_evaluated; uint64_t n_rows, rows_usable;
+    const int64_t* ll; const uint64_t* counts;               /* [n_cols][n_hyp] x 2^24, [n_cols][3]: as vtx_donor_ll_get */
+    const uint16_t* grid_permille; const int64_t* grid_objective; const uint64_t* grid_calls;   /* [n_evaluated], ascending m; calls [.][3] */
+    const uint64_t* row_alt; const uint64_t* row_depth;       /* [n_rows]: A_v, T_v */
+} vtx_ambient;
+int         vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                               const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const uint8_t* dosage,
+                               const vtx_ambient_params* params, vtx_ambient* out);
+
 /* Injective code of a cell-barcode tag of the form [ACGT]{1,24}(-N)? with N = 1..99 written without a leading zero:
  * 2 bits per base, 5 bits length, 7 bits N (0 = no suffix); < 2^60.  Returns VTX_NO_CB_KEY if the bytes have another
  * form -- the caller then lists them as an exotic tag (VTX_CB_EXOTIC | i). */

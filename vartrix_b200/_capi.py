@@ -32,7 +32,7 @@ SYMBOLS = [
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
     "vtx_set_min_base_quality", "vtx_bam_low_base_quality", "vtx_set_locus_stats", "vtx_locus_stats_get",
-    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells",
+    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells", "vtx_donors_ambient",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
 CB_EXOTIC = 0x8000000000000000
@@ -116,6 +116,18 @@ class Clusters(C.Structure):       # vtx_clusters
                 ("n_rows", C.c_uint64), ("rows_used", C.c_uint64), ("ll", C.POINTER(C.c_int64)), ("counts", C.POINTER(C.c_uint64)),
                 ("row_used", C.POINTER(C.c_uint8)), ("alt_w", C.POINTER(C.c_int64)), ("depth_w", C.POINTER(C.c_int64)),
                 ("restart_score", C.POINTER(C.c_int64)), ("restart_iters", C.POINTER(C.c_uint32))]
+
+
+class AmbientParams(C.Structure):  # vtx_ambient_params
+    _fields_ = [("n_donors", C.c_uint32), ("error_rate", C.c_double), ("rho_permille", C.c_int32), ("grid_batch", C.c_uint32)]
+
+
+class Ambient(C.Structure):        # vtx_ambient
+    _fields_ = [("n_donors", C.c_uint32), ("n_cols", C.c_uint32), ("n_hyp", C.c_uint32), ("rho_permille", C.c_uint32),
+                ("n_evaluated", C.c_uint32), ("n_rows", C.c_uint64), ("rows_usable", C.c_uint64),
+                ("ll", C.POINTER(C.c_int64)), ("counts", C.POINTER(C.c_uint64)), ("grid_permille", C.POINTER(C.c_uint16)),
+                ("grid_objective", C.POINTER(C.c_int64)), ("grid_calls", C.POINTER(C.c_uint64)),
+                ("row_alt", C.POINTER(C.c_uint64)), ("row_depth", C.POINTER(C.c_uint64))]
 
 
 class Metrics(C.Structure):
@@ -204,6 +216,9 @@ def load():
     L.vtx_cluster_cells.restype = C.c_int
     L.vtx_cluster_cells.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                                     C.POINTER(ClusterParams), C.POINTER(Clusters)]
+    L.vtx_donors_ambient.restype = C.c_int
+    L.vtx_donors_ambient.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                     C.c_void_p, C.POINTER(AmbientParams), C.POINTER(Ambient)]
     L.vtx_pack_cb.restype = C.c_uint64
     L.vtx_pack_cb.argtypes = [C.c_char_p, C.c_uint32]
     L.vtx_gather_start.restype = C.c_int

@@ -26,6 +26,7 @@
 #include "stager.hpp"
 #include "../vtx_donors.cuh"
 #include "../vtx_clusters.cuh"
+#include "../vtx_ambient.cuh"
 
 using namespace vtxhost;
 
@@ -56,6 +57,8 @@ struct Opts {
     std::string out_donors, donors;            // --out-donors FILE, --donors NAME,NAME,...
     double donor_error_rate = 0.01;            // --donor-error-rate
     bool donor_error_rate_given = false;
+    std::string ambient_rna, out_ambient;      // --ambient-rna MODE, --out-ambient FILE
+    int32_t ambient_permille = -1;             // the fraction of --ambient-rna in thousandths; -1: estimate
     std::string out_clusters, out_cluster_alleles;     // --out-clusters FILE, --out-cluster-alleles FILE
     uint32_t clusters = 0, cluster_restarts = 8;       // --clusters K, --cluster-restarts R
     uint64_t cluster_seed = 0;                         // --cluster-seed S
@@ -84,6 +87,10 @@ void usage()
          "                              doublet log-likelihoods from the cell's REF / ALT counts, the best pair and the call\n"
          "      --donors LIST           The VCF samples that are the pool's donors, e.g. S1,S4,S2 (2 to 32) [every sample]\n"
          "      --donor-error-rate E    Per-molecule error rate of the donor model, 1e-6 .. 0.25 [0.01]\n"
+         "      --ambient-rna MODE      With --out-donors: model ambient RNA, molecules from the whole pool mixed into every cell.\n"
+         "                              MODE is 'estimate' (the fraction that fits the cells best) or a fraction 0 .. 0.5 with at\n"
+         "                              most three decimals\n"
+         "      --out-ambient FILE      With --ambient-rna: the fit of every fraction evaluated (TSV: rho, objective, calls)\n"
          "      --out-clusters FILE     Cluster the cells into --clusters donors without genotypes (TSV, one line per barcode, the\n"
          "                              --out-donors columns with clusters C0, C1, ... for donors): allele-fraction EM, doublet calls\n"
          "      --clusters K            Number of clusters, 2 .. 32 (needed by --out-clusters)\n"
@@ -139,6 +146,20 @@ bool parse_devices(const std::string& spec, std::vector<int>* out)
     return !out->empty();
 }
 
+// --ambient-rna: "estimate" (-1), or a fraction 0 .. 0.5 with at most three decimals, in thousandths
+bool parse_ambient(const std::string& s, int32_t* permille)
+{
+    if (s == "estimate") { *permille = -1; return true; }
+    const size_t dot = s.find('.');
+    const std::string whole = s.substr(0, dot), frac = dot == std::string::npos ? "" : s.substr(dot + 1);
+    if (whole.empty() || whole.size() > 3 || (dot != std::string::npos && (frac.empty() || frac.size() > 3))) return false;
+    for (const char c : whole + frac) if (!isdigit((unsigned char)c)) return false;
+    const long m = atol(whole.c_str()) * 1000 + (frac.empty() ? 0 : atol((frac + std::string(3 - frac.size(), '0')).c_str()));
+    if (m > vtx::ambient::kMaxPermille) return false;
+    *permille = int32_t(m);
+    return true;
+}
+
 bool parse(int argc, char** argv, Opts* o)
 {
     auto need = [&](int& i) -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: %s needs a value\n", argv[i]); exit(1); } return argv[++i]; };
@@ -168,6 +189,15 @@ bool parse(int argc, char** argv, Opts* o)
             o->donor_error_rate = x;
             o->donor_error_rate_given = true;
         }
+        else if (a == "--ambient-rna") {
+            o->ambient_rna = v();
+            if (!parse_ambient(o->ambient_rna, &o->ambient_permille)) {
+                fprintf(stderr, "error: --ambient-rna must be 'estimate' or a fraction from 0 to 0.5 with at most three decimals, not '%s'\n",
+                        o->ambient_rna.c_str());
+                return false;
+            }
+        }
+        else if (a == "--out-ambient") o->out_ambient = v();
         else if (a == "--out-clusters") o->out_clusters = v();
         else if (a == "--out-cluster-alleles") o->out_cluster_alleles = v();
         else if (a == "--clusters" || a == "--cluster-restarts" || a == "--cluster-seed") {
@@ -230,12 +260,24 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --out-variant-stats counts what the GPU run scores: it cannot be combined with --dump-staged\n");
         return false;
     }
+    if (!o->ambient_rna.empty() && !o->dump_staged.empty()) {
+        fprintf(stderr, "error: --ambient-rna models what the GPU run counts: it cannot be combined with --dump-staged\n");
+        return false;
+    }
     if (!o->out_donors.empty() && !o->dump_staged.empty()) {
         fprintf(stderr, "error: --out-donors sums what the GPU run counts: it cannot be combined with --dump-staged\n");
         return false;
     }
     if (o->out_donors.empty() && (!o->donors.empty() || o->donor_error_rate_given)) {
         fprintf(stderr, "error: --donors and --donor-error-rate only apply with --out-donors\n");
+        return false;
+    }
+    if (!o->ambient_rna.empty() && o->out_donors.empty()) {
+        fprintf(stderr, "error: --ambient-rna only applies with --out-donors\n");
+        return false;
+    }
+    if (!o->out_ambient.empty() && o->ambient_rna.empty()) {
+        fprintf(stderr, "error: --out-ambient only applies with --ambient-rna\n");
         return false;
     }
     if (o->out_clusters.empty() != (o->clusters == 0)) {
@@ -272,6 +314,7 @@ void check_inputs_exist(const Opts& o)
     if (o.dump_staged.empty()) { validate_output_path(o.out_matrix); validate_output_path(o.ref_matrix); }
     if (!o.out_variant_stats.empty()) validate_output_path(o.out_variant_stats);
     if (!o.out_donors.empty()) validate_output_path(o.out_donors);
+    if (!o.out_ambient.empty()) validate_output_path(o.out_ambient);
     if (!o.out_clusters.empty()) validate_output_path(o.out_clusters);
     if (!o.out_cluster_alleles.empty()) validate_output_path(o.out_cluster_alleles);
     if (!exists(o.fasta + ".fai")) { LOG_ERR("File %s.fai does not exist", o.fasta.c_str()); exit(1); }
@@ -467,7 +510,6 @@ bool write_donors(const std::string& path, const std::vector<std::string>& barco
 {
     using namespace vtx::donors;
     const uint32_t D = uint32_t(names.size()), H = n_hyp(D);
-    const int64_t T = 5 * int64_t(kScale);
     FILE* f = fopen(path.c_str(), "wb");
     if (!f) return false;
     fputs("barcode\tvariants\tref\talt\tcall\tassignment\tsinglet_llr\tdoublet_llr\tbest_singlet\tsecond_singlet\tbest_doublet", f);
@@ -483,7 +525,7 @@ bool write_donors(const std::string& path, const std::vector<std::string>& barco
         for (uint32_t h = second + 1; h < D; ++h) if (h != best && L[h] > L[second]) second = h;
         for (uint32_t h = D + 1; h < H; ++h) if (L[h] > L[pair]) pair = h;
         const int64_t s_llr = L[best] - L[second], d_llr = L[pair] - L[best];
-        const int call = n[0] == 0 ? 2 : d_llr >= T ? 1 : s_llr >= T ? 0 : 2;        // singlet, doublet, unassigned
+        const uint32_t call = call_of(n[0], L[best], L[second], L[pair]);           // singlet, doublet, unassigned
         ++calls[call];
         const std::string assignment = call == 0 ? names[best] : call == 1 ? pair_name(pair) : ".";
         fprintf(f, "%s\t%llu\t%llu\t%llu\t%s\t%s\t%.6f\t%.6f\t%s\t%s\t%s", barcodes[c].c_str(), (unsigned long long)n[0],
@@ -492,6 +534,20 @@ bool write_donors(const std::string& path, const std::vector<std::string>& barco
                 pair_name(pair).c_str());
         for (uint32_t d = 0; d < D; ++d) fprintf(f, "\t%.6f", double(L[d]) / kScale);
         fputc('\n', f);
+    }
+    return fclose(f) == 0;
+}
+
+// --out-ambient: one line per evaluated fraction, ascending; the objective J / 2^24 and the calls at that fraction
+bool write_ambient(const std::string& path, const vtx_ambient& am)
+{
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    fputs("rho\tobjective\tsinglet\tdoublet\tunassigned\tchosen\n", f);
+    for (uint32_t i = 0; i < am.n_evaluated; ++i) {
+        const uint64_t* c = am.grid_calls + 3 * size_t(i);
+        fprintf(f, "%.3f\t%.6f\t%llu\t%llu\t%llu\t%d\n", am.grid_permille[i] / 1000.0, double(am.grid_objective[i]) / vtx::donors::kScale,
+                (unsigned long long)c[0], (unsigned long long)c[1], (unsigned long long)c[2], int(am.grid_permille[i] == am.rho_permille));
     }
     return fclose(f) == 0;
 }
@@ -566,6 +622,7 @@ int main(int argc, char** argv)
     // --out-donors: the VCF (with its sample columns) is read before any GPU work, so that a bad donor list is refused first
     std::vector<VcfRecord> recs;
     const bool with_donors = !o.out_donors.empty();
+    const bool with_ambient = !o.ambient_rna.empty();      // the donors are scored once, after the finish, over the result
     DonorTable donors;
     if (with_donors) {
         VcfGenotypes gts;
@@ -588,15 +645,15 @@ int main(int argc, char** argv)
                 vtx_config cfg{};
                 cfg.device = cuda_index[d];
                 cfg.mode = o.scoring == "consensus" ? VTX_MODE_CONSENSUS : o.scoring == "coverage" ? VTX_MODE_COVERAGE : VTX_MODE_ALT_FRAC;
-                // the matrix writers need row, col and the values only; --out-clusters also needs the REF / ALT counts
-                cfg.flags = o.out_clusters.empty() ? VTX_F_VALUES_ONLY : 0u;
+                // the matrix writers need row, col and the values only; --out-clusters and --ambient-rna also need the REF / ALT counts
+                cfg.flags = o.out_clusters.empty() && !with_ambient ? VTX_F_VALUES_ONLY : 0u;
                 if (o.collapse_mates) cfg.flags |= VTX_F_NAME_KEYS;      // name keys through the UMI collapse
                 cfg.use_umi = o.umi || o.collapse_mates; cfg.match = 1; cfg.mismatch = -5; cfg.gap_open = -5; cfg.gap_extend = -1; cfg.min_score = 25;
                 cfg.band_k = 6; cfg.band_w = 20; cfg.band_mode = VTX_BAND_FULL;          // main.rs:33-34
                 if (vtx_create(&cfg, &ln.ctx) != VTX_OK) { ln.err = vtx_last_error(nullptr); return 1; }
                 if (o.min_base_quality && vtx_set_min_base_quality(ln.ctx, o.min_base_quality) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
                 if (!o.out_variant_stats.empty() && vtx_set_locus_stats(ln.ctx, 1) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
-                if (with_donors && vtx_set_donors(ln.ctx, uint32_t(donors.names.size()), recs.size(), donors.dosage.data(), o.donor_error_rate) != VTX_OK) {
+                if (with_donors && !with_ambient && vtx_set_donors(ln.ctx, uint32_t(donors.names.size()), recs.size(), donors.dosage.data(), o.donor_error_rate) != VTX_OK) {
                     ln.err = vtx_last_error(ln.ctx); return 1;
                 }
                 if (vtx_set_barcodes(ln.ctx, bcs.bytes.data(), bcs.off.data(), uint32_t(bcs.keys.size())) != VTX_OK) { ln.err = vtx_last_error(ln.ctx); return 1; }
@@ -793,7 +850,7 @@ int main(int argc, char** argv)
         return true;
     };
     auto take_donors = [&](Lane& ln) -> bool {         // --out-donors: right after the lane's finish
-        if (!with_donors) return true;
+        if (!with_donors || with_ambient) return true;
         const int64_t* ll = nullptr; const uint64_t* cnt = nullptr; uint32_t nc = 0, nh = 0;
         if (vtx_donor_ll_get(ln.ctx, &ll, &cnt, &nc, &nh) != VTX_OK) return false;
         ln.donor_ll.assign(ll, ll + size_t(nc) * nh);
@@ -964,18 +1021,43 @@ int main(int argc, char** argv)
         }
         if (!write_variant_stats(o.out_variant_stats, recs, dev, host_rows, host_filters)) { LOG_ERR("error writing variant statistics file"); rc = 1; }
     }
-    if (with_donors) {                  // the lanes' int64 sums add up to the one-GPU sums exactly
+    vtx_ambient am{};
+    if (with_ambient) {                 // once, on lane 0, over every lane's triplets
+        const vtx_ambient_params ap{ uint32_t(donors.names.size()), o.donor_error_rate, o.ambient_permille, 0 };
+        if (vtx_donors_ambient(ctx, res.n, res.row, res.col, res.ref_cnt, res.alt_cnt, recs.size(), uint32_t(bcs.keys.size()), donors.dosage.data(),
+                               &ap, &am) != VTX_OK) {
+            printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx)); rc = 1;
+        }
+    }
+    if (with_donors && (!with_ambient || rc == 0)) {
         validate_output_path(o.out_donors);
         const size_t H = vtx::donors::n_hyp(uint32_t(donors.names.size()));
         std::vector<int64_t> ll(bcs.keys.size() * H, 0);
         std::vector<uint64_t> cnt(bcs.keys.size() * 3, 0);
-        for (const Lane& ln : lanes) {
-            if (ln.donor_ll.size() != ll.size() || ln.donor_cnt.size() != cnt.size()) { LOG_ERR("donor sums of GPU %d have the wrong size", ln.device); rc = 1; continue; }
-            for (size_t i = 0; i < ll.size(); ++i) ll[i] += ln.donor_ll[i];
-            for (size_t i = 0; i < cnt.size(); ++i) cnt[i] += ln.donor_cnt[i];
+        if (with_ambient) {
+            ll.assign(am.ll, am.ll + ll.size());
+            cnt.assign(am.counts, am.counts + cnt.size());
+        } else {
+            for (const Lane& ln : lanes) {          // the lanes' int64 sums add up to the one-GPU sums exactly
+                if (ln.donor_ll.size() != ll.size() || ln.donor_cnt.size() != cnt.size()) { LOG_ERR("donor sums of GPU %d have the wrong size", ln.device); rc = 1; continue; }
+                for (size_t i = 0; i < ll.size(); ++i) ll[i] += ln.donor_ll[i];
+                for (size_t i = 0; i < cnt.size(); ++i) cnt[i] += ln.donor_cnt[i];
+            }
         }
         uint64_t calls[3] = { 0, 0, 0 };
         if (!write_donors(o.out_donors, bcs.keys, donors.names, ll, cnt, calls)) { LOG_ERR("error writing donor file"); rc = 1; }
+        if (with_ambient) {
+            if (!o.out_ambient.empty()) {
+                validate_output_path(o.out_ambient);
+                if (!write_ambient(o.out_ambient, am)) { LOG_ERR("error writing ambient file"); rc = 1; }
+            }
+            std::string at_zero;
+            for (uint32_t i = 0; i < am.n_evaluated; ++i)
+                if (am.grid_permille[i] == 0) at_zero = std::to_string(am.grid_calls[3 * size_t(i) + 1]) + " at rho 0.000, ";
+            LOG_INFO("Ambient RNA: rho %.3f (%s); fractions evaluated: %u; doublets: %s%llu at rho %.3f", am.rho_permille / 1000.0,
+                     o.ambient_permille < 0 ? "estimated" : "given", am.n_evaluated, at_zero.c_str(), (unsigned long long)calls[1],
+                     am.rho_permille / 1000.0);
+        }
         std::string list;
         for (const std::string& n : donors.names) list += (list.empty() ? "" : ",") + n;
         LOG_INFO("Donors: %zu (%s), error rate %g; rows with a genotype for every donor: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",

@@ -9,6 +9,7 @@
 #include "vtx_locus_stats.cuh"
 #include "vtx_donors.cuh"
 #include "vtx_clusters.cuh"
+#include "vtx_ambient.cuh"
 
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
@@ -156,7 +157,13 @@ struct vtx_ctx {
     std::vector<uint64_t> h_cl_cnt;
     std::vector<uint8_t> h_cl_used;
     std::vector<uint32_t> h_cl_iters;
-    HostBuf h_stage;                                   // scalars read back between the staging phases
+    // vtx_donors_ambient: device work buffers (the entries and their by-cell index live in the cl_* buffers above) and the
+    // host outputs of the last call
+    DBuf am_sums, am_tix, am_touched, am_dos, am_tab, am_grid;
+    std::vector<int64_t> h_am_ll, h_am_obj;
+    std::vector<uint64_t> h_am_cnt, h_am_calls, h_am_alt, h_am_depth;
+    std::vector<uint16_t> h_am_m;
+    HostBuf h_stage;                                  // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
 
@@ -1070,6 +1077,32 @@ int submit_resident(vtx_ctx* ctx, const Batch* db, const char* fn, uint32_t max_
 
 void comm_destroy(vtx_ctx* ctx);      // with the NCCL loader below
 
+// The count entries vtx_cluster_cells and vtx_donors_ambient take, validated in one pass: row < n_rows, col < n_cols, (row, col)
+// strictly ascending, and at most max_molecules REF + ALT molecules per row (`why` says what a larger sum would break).  Rows are
+// contiguous, so per_row(v, i0, i1, molecules) sees each row present once, with its entries [i0, i1).
+template <typename PerRow>
+int validate_entries(vtx_ctx* ctx, const char* fn, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                            const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, uint64_t max_molecules, const char* why, PerRow per_row)
+{
+    for (uint64_t i = 0; i < n;) {
+        const uint32_t v = row[i];
+        if (v >= n_rows) return set_err(ctx, VTX_E_INVALID, "%s: entry %llu has row %u >= n_rows %llu", fn, (unsigned long long)i, v, (unsigned long long)n_rows);
+        if (i && v < row[i - 1]) return set_err(ctx, VTX_E_INVALID, "%s: entry %llu: rows are not ascending", fn, (unsigned long long)i);
+        uint64_t molecules = 0;
+        const uint64_t i0 = i;
+        for (; i < n && row[i] == v; ++i) {
+            if (col[i] >= n_cols) return set_err(ctx, VTX_E_INVALID, "%s: entry %llu has col %u >= n_cols %u", fn, (unsigned long long)i, col[i], n_cols);
+            if (i > i0 && col[i] <= col[i - 1])
+                return set_err(ctx, VTX_E_INVALID, "%s: entry %llu: (row, col) is not strictly ascending", fn, (unsigned long long)i);
+            molecules += uint64_t(ref_cnt[i]) + alt_cnt[i];
+            if (molecules > max_molecules)
+                return set_err(ctx, VTX_E_INVALID, "%s: row %u holds more than %llu molecules; %s", fn, v, (unsigned long long)max_molecules, why);
+        }
+        per_row(v, i0, i, molecules);
+    }
+    return VTX_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -1593,27 +1626,14 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
     ctx->h_cl_used.assign(size_t(n_rows), 0);
     std::vector<uint32_t> used_rows;
     const uint64_t kMaxMolecules = ((1ull << 53) - (1ull << 17)) >> 16;     // molecules x 2^16 + 2^17 stays below 2^53
-    for (uint64_t i = 0; i < n;) {
-        const uint32_t v = row[i];
-        if (v >= n_rows) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu has row %u >= n_rows %llu", (unsigned long long)i, v, (unsigned long long)n_rows);
-        if (i && v < row[i - 1]) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu: rows are not ascending", (unsigned long long)i);
+    int vrc = validate_entries(ctx, "vtx_cluster_cells", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxMolecules,
+                               "its weighted sums would not be exact", [&](uint32_t v, uint64_t i0, uint64_t i1, uint64_t) {
         uint32_t with_ref = 0, with_alt = 0;
-        uint64_t molecules = 0;
-        const uint64_t i0 = i;
-        for (; i < n && row[i] == v; ++i) {
-            if (col[i] >= n_cols) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu has col %u >= n_cols %u", (unsigned long long)i, col[i], n_cols);
-            if (i > i0 && col[i] <= col[i - 1])
-                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: entry %llu: (row, col) is not strictly ascending", (unsigned long long)i);
-            with_ref += ref_cnt[i] > 0;
-            with_alt += alt_cnt[i] > 0;
-            molecules += uint64_t(ref_cnt[i]) + alt_cnt[i];
-            if (molecules > kMaxMolecules)
-                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: row %u holds more than %llu molecules; its weighted sums would not be exact", v,
-                               (unsigned long long)kMaxMolecules);
-        }
-        row_start[size_t(v) + 1] = uint32_t(i - i0);
+        for (uint64_t i = i0; i < i1; ++i) { with_ref += ref_cnt[i] > 0; with_alt += alt_cnt[i] > 0; }
+        row_start[size_t(v) + 1] = uint32_t(i1 - i0);
         if (with_ref >= kMinCells && with_alt >= kMinCells) { ctx->h_cl_used[v] = 1; used_rows.push_back(v); }
-    }
+    });
+    if (vrc) return vrc;
     for (uint64_t v = 0; v < n_rows; ++v) row_start[v + 1] += row_start[v];
 
     cudaStream_t st = ctx->stream;
@@ -1757,6 +1777,225 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
     out->ll = ctx->h_cl_ll.data(); out->counts = ctx->h_cl_cnt.data(); out->row_used = ctx->h_cl_used.data();
     out->alt_w = ctx->h_cl_A.data(); out->depth_w = ctx->h_cl_T.data();
     out->restart_score = ctx->h_cl_score.data(); out->restart_iters = ctx->h_cl_iters.data();
+    return VTX_OK;
+}
+
+int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                       const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const uint8_t* dosage,
+                       const vtx_ambient_params* params, vtx_ambient* out)
+{
+    using namespace ambient;
+    if (!ctx || !params || !out) return VTX_E_INVALID;
+    *out = vtx_ambient{};
+    if (!ctx->finished || ctx->gather_pending)
+        return set_err(ctx, VTX_E_STATE, "vtx_donors_ambient: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const uint32_t D = params->n_donors;
+    const int32_t given = params->rho_permille;
+    if (D < donors::kMinDonors || D > donors::kMaxDonors)
+        return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: %u donors; 2 to 32 are supported", D);
+    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
+        return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: error rate %g outside [1e-6, 0.25]", params->error_rate);
+    if (given < -1 || given > kMaxPermille)
+        return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: rho_permille %d; -1 (estimate) or 0 to 500", given);
+    if (n && (!row || !col || !ref_cnt || !alt_cnt)) return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: an entry array is NULL");
+    if (n_rows && !dosage) return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: dosage is NULL");
+    if (n > 0xFFFFFFFFull || n_rows > 0xFFFFFFFFull)
+        return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: %llu entries over %llu rows; both must be below 2^32",
+                       (unsigned long long)n, (unsigned long long)n_rows);
+    const uint32_t H = donors::n_hyp(D);
+    // device memory, before any host table of n_rows entries: the entries (16 B) and their by-cell copy (12 B); per row the used
+    // flag, the touched index and A, T; per cell the index, the log-likelihoods and the counts.  One m's tables come below.
+    // every buffer is allocated with 1/8 to spare (ensure), so both checks and the pass size count that margin
+    constexpr double kSlack = 1.125;
+    const double need = (double(n) * 28 + double(n_rows) * 21 + double(n_cols) * (8 + 24 + 8.0 * H)) * kSlack;
+    double avail = 0;
+    {
+        CK(cudaSetDevice(ctx->device));
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        size_t held = 0;
+        for (DBuf* b : { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_cell_count, &ctx->cl_cell_start,
+                         &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_ll, &ctx->cl_cnt, &ctx->am_sums, &ctx->am_tix,
+                         &ctx->am_touched, &ctx->am_dos, &ctx->am_tab, &ctx->am_grid })
+            held += b->cap;
+        avail = double(free_b) + double(held);
+        if (need > avail)
+            return set_err(ctx, VTX_E_NOMEM, "vtx_donors_ambient needs %.0f MB of device memory, %.0f MB are free", need * 1e-6, avail * 1e-6);
+    }
+    const size_t cells = size_t(n_rows) * D;
+    for (size_t i = 0; i < cells; ++i)
+        if (dosage[i] > 2 && dosage[i] != donors::kMissing)
+            return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: dosage %u at row %zu, donor %zu (0, 1, 2 or VTX_GT_MISSING)",
+                           unsigned(dosage[i]), i / D, i % D);
+    std::vector<uint8_t> usable(size_t(n_rows) + 1, 0);
+    uint64_t rows_usable = 0;
+    for (uint64_t v = 0; v < n_rows; ++v) rows_usable += usable[v] = donors::row_usable(dosage + size_t(v) * D, D) ? 1 : 0;
+    // validate the entries in one pass; a usable row with an entry of r + a > 0 is "touched" and gets the next table index
+    std::vector<uint32_t> tix(size_t(n_rows) + 1, 0), touched;
+    int rc = validate_entries(ctx, "vtx_donors_ambient", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxRowDepth,
+                              "its pool fraction would not be exact", [&](uint32_t v, uint64_t, uint64_t, uint64_t depth) {
+        if (depth && usable[v]) { tix[v] = uint32_t(touched.size()); touched.push_back(v); }
+    });
+    if (rc) return rc;
+    const uint32_t n_t = uint32_t(touched.size());
+    std::vector<uint8_t> dos(size_t(n_t) * D + 1);
+    for (uint32_t t = 0; t < n_t; ++t) memcpy(dos.data() + size_t(t) * D, dosage + size_t(touched[t]) * D, D);
+    // the rest of the memory holds the tables of as many m as fit, at least one
+    const double fixed = need + double(n_t) * (D + 4) * kSlack, per_m = double(n_t) * 40 * kSlack;
+    if (fixed + per_m > avail)
+        return set_err(ctx, VTX_E_NOMEM, "vtx_donors_ambient needs %.0f MB of device memory, %.0f MB are free", (fixed + per_m) * 1e-6, avail * 1e-6);
+    uint32_t batch = kMaxBatch;
+    if (per_m > 0) batch = uint32_t(std::min(double(kMaxBatch), std::floor((avail - fixed) / per_m)));
+    if (params->grid_batch) batch = std::min(batch, params->grid_batch);
+
+    cudaStream_t st = ctx->stream;
+    const size_t nb = size_t(n) * 4 + 4;
+    ENS(ctx->cl_row, nb); ENS(ctx->cl_col, nb); ENS(ctx->cl_r, nb); ENS(ctx->cl_a, nb);
+    ENS(ctx->cl_c_row, nb); ENS(ctx->cl_c_r, nb); ENS(ctx->cl_c_a, nb);
+    ENS(ctx->cl_used, usable.size());
+    ENS(ctx->am_tix, tix.size() * 4);
+    ENS(ctx->am_touched, size_t(n_t) * 4 + 4);
+    ENS(ctx->am_dos, dos.size());
+    ENS(ctx->am_sums, size_t(n_rows) * 16 + 16);
+    ENS(ctx->cl_cell_count, (size_t(n_cols) + 1) * 4);
+    ENS(ctx->cl_cell_start, (size_t(n_cols) + 1) * 4);
+    ENS(ctx->cl_ll, size_t(n_cols) * H * 8 + 8); ENS(ctx->cl_cnt, size_t(n_cols) * 24 + 8);
+    ENS(ctx->am_tab, size_t(batch) * n_t * 40 + 8);
+    ENS(ctx->am_grid, size_t(kMaxBatch) * 4 * 8);
+    if (n) {
+        CK(cudaMemcpyAsync(ctx->cl_row.p, row, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_r.p, ref_cnt, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_a.p, alt_cnt, n * 4, cudaMemcpyHostToDevice, st));
+    }
+    CK(cudaMemcpyAsync(ctx->cl_used.p, usable.data(), usable.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->am_tix.p, tix.data(), tix.size() * 4, cudaMemcpyHostToDevice, st));
+    if (n_t) {
+        CK(cudaMemcpyAsync(ctx->am_touched.p, touched.data(), size_t(n_t) * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->am_dos.p, dos.data(), size_t(n_t) * D, cudaMemcpyHostToDevice, st));
+    }
+    unsigned long long* d_A = P<unsigned long long>(ctx->am_sums);
+    unsigned long long* d_T = d_A + n_rows;
+    CK(cudaMemsetAsync(ctx->am_sums.p, 0, size_t(n_rows) * 16, st));
+
+    // A_v, T_v and the by-cell index of the kept entries (§5g's kernels with used = the usable rows)
+    const uint32_t nn = uint32_t(n);
+    const unsigned egrid = std::max(1u, std::min(blocks_for(n, kAmThreads), unsigned(ctx->n_sm) * 16));
+    if (n) {
+        vtx_k_am_rowsum<<<egrid, kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a), d_A, d_T);
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    clusters::vtx_k_cl_count<<<egrid, kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                  P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_count));
+    CK(cudaGetLastError());
+    rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->cl_cell_count), n_cols, P<uint32_t>(ctx->cl_cell_start), nullptr);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    clusters::vtx_k_cl_scatter<<<egrid, kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                    P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_start),
+                                                    P<uint32_t>(ctx->cl_cell_count), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r),
+                                                    P<uint32_t>(ctx->cl_c_a));
+    CK(cudaGetLastError());
+    const clusters::CellEntries ce{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
+
+    // J(m) and the calls of every m in `ms`, `batch` m per pass; with `final` (one m), also the cells' log-likelihoods
+    const Fractions fr = fractions(params->error_rate);
+    unsigned long long* d_J = P<unsigned long long>(ctx->am_grid);
+    unsigned long long* d_calls = d_J + kMaxBatch;
+    std::vector<unsigned long long> h_grid(size_t(kMaxBatch) * 4);
+    auto evaluate = [&](const std::vector<uint16_t>& ms, bool final, std::vector<int64_t>* J, std::vector<uint64_t>* calls) -> int {
+        for (size_t o = 0; o < ms.size(); o += batch) {
+            Batch bt{};
+            bt.n = uint32_t(std::min<size_t>(batch, ms.size() - o));
+            for (uint32_t b = 0; b < bt.n; ++b) bt.m[b] = ms[o + b];
+            CK(cudaMemsetAsync(ctx->am_grid.p, 0, h_grid.size() * 8, st));
+            if (n_t) {
+                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_t, kAmThreads), unsigned(ctx->n_sm) * 16));
+                vtx_k_am_tables<<<g, kAmThreads, 0, st>>>(bt, fr, n_t, P<uint32_t>(ctx->am_touched), d_A, d_T, P<int32_t>(ctx->am_tab));
+                CK(cudaGetLastError());
+            }
+            if (n_cols) {
+                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_cols * 32, kAmThreads), unsigned(ctx->n_sm) * 16));
+                const uint32_t* tx = P<uint32_t>(ctx->am_tix);
+                const uint8_t* dd = P<uint8_t>(ctx->am_dos);
+                const int32_t* tb = P<int32_t>(ctx->am_tab);
+                int64_t* ll = final ? P<int64_t>(ctx->cl_ll) : nullptr;
+                uint64_t* cnt = final ? P<uint64_t>(ctx->cl_cnt) : nullptr;
+                if (H <= 32) vtx_k_am_score<1><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
+                else if (H <= 64) vtx_k_am_score<2><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
+                else if (H <= 160) vtx_k_am_score<5><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
+                else if (H <= 288) vtx_k_am_score<9><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
+                else vtx_k_am_score<17><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
+                CK(cudaGetLastError());
+            }
+            CK(cudaMemcpyAsync(h_grid.data(), ctx->am_grid.p, h_grid.size() * 8, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            for (uint32_t b = 0; b < bt.n; ++b) {
+                J->push_back(int64_t(h_grid[b]));
+                for (int k = 0; k < 3; ++k) calls->push_back(h_grid[kMaxBatch + 3 * size_t(b) + k]);
+            }
+        }
+        return VTX_OK;
+    };
+    // the estimate: the coarse grid, then every m within kFineReach of its winner; the largest J wins, ties the smallest m
+    std::vector<uint16_t> ms;
+    std::vector<int64_t> obj;
+    std::vector<uint64_t> calls;
+    auto best_of = [&]() {
+        size_t w = 0;
+        for (size_t i = 1; i < ms.size(); ++i)
+            if (obj[i] > obj[w] || (obj[i] == obj[w] && ms[i] < ms[w])) w = i;
+        return ms[w];
+    };
+    uint32_t chosen = uint32_t(given);
+    if (given < 0) {
+        for (uint32_t m = 0; m <= uint32_t(kMaxPermille); m += kCoarseStep) ms.push_back(uint16_t(m));
+        rc = evaluate(ms, false, &obj, &calls);
+        if (rc) return rc;
+        const uint32_t mc = best_of();
+        std::vector<uint16_t> fine;
+        for (uint32_t m = mc > kFineReach ? mc - kFineReach : 0; m <= std::min<uint32_t>(kMaxPermille, mc + kFineReach); ++m)
+            if (m % kCoarseStep) fine.push_back(uint16_t(m));
+        rc = evaluate(fine, false, &obj, &calls);
+        if (rc) return rc;
+        ms.insert(ms.end(), fine.begin(), fine.end());
+        chosen = best_of();
+    }
+    std::vector<int64_t> obj_f;
+    std::vector<uint64_t> calls_f;
+    rc = evaluate({ uint16_t(chosen) }, true, &obj_f, &calls_f);
+    if (rc) return rc;
+    if (given >= 0) { ms.assign(1, uint16_t(chosen)); obj = obj_f; calls = calls_f; }
+    std::vector<size_t> order(ms.size());
+    for (size_t i = 0; i < order.size(); ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](size_t x, size_t y) { return ms[x] < ms[y]; });
+    ctx->h_am_m.resize(ms.size()); ctx->h_am_obj.resize(ms.size()); ctx->h_am_calls.resize(ms.size() * 3);
+    for (size_t i = 0; i < order.size(); ++i) {
+        ctx->h_am_m[i] = ms[order[i]];
+        ctx->h_am_obj[i] = obj[order[i]];
+        for (int k = 0; k < 3; ++k) ctx->h_am_calls[3 * i + k] = calls[3 * order[i] + k];
+    }
+
+    ctx->h_am_ll.resize(size_t(n_cols) * H);
+    ctx->h_am_cnt.resize(size_t(n_cols) * 3);
+    ctx->h_am_alt.resize(size_t(n_rows));
+    ctx->h_am_depth.resize(size_t(n_rows));
+    if (n_cols) {
+        CK(cudaMemcpyAsync(ctx->h_am_ll.data(), ctx->cl_ll.p, ctx->h_am_ll.size() * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_am_cnt.data(), ctx->cl_cnt.p, ctx->h_am_cnt.size() * 8, cudaMemcpyDeviceToHost, st));
+    }
+    if (n_rows) {
+        CK(cudaMemcpyAsync(ctx->h_am_alt.data(), d_A, size_t(n_rows) * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_am_depth.data(), d_T, size_t(n_rows) * 8, cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+
+    out->n_donors = D; out->n_cols = n_cols; out->n_hyp = H; out->rho_permille = chosen; out->n_evaluated = uint32_t(ms.size());
+    out->n_rows = n_rows; out->rows_usable = rows_usable;
+    out->ll = ctx->h_am_ll.data(); out->counts = ctx->h_am_cnt.data();
+    out->grid_permille = ctx->h_am_m.data(); out->grid_objective = ctx->h_am_obj.data(); out->grid_calls = ctx->h_am_calls.data();
+    out->row_alt = ctx->h_am_alt.data(); out->row_depth = ctx->h_am_depth.data();
     return VTX_OK;
 }
 

@@ -109,6 +109,14 @@ VTX_DN_HD inline void add_slot(const Inputs& in, uint32_t q, int64_t* ll, uint64
     cnt[0] += 1; cnt[1] += r; cnt[2] += a;
 }
 
+// the call of a cell with `variants` rows from its best singlet, best other singlet and best doublet log-likelihoods:
+// 0 singlet, 1 doublet, 2 unassigned, with the threshold T = 5 nats in the integer scale
+VTX_DN_HD inline uint32_t call_of(uint64_t variants, int64_t best, int64_t second, int64_t pair)
+{
+    const int64_t T = 5 * int64_t(kScale);
+    return variants == 0 ? 2u : pair - best >= T ? 1u : best - second >= T ? 0u : 2u;
+}
+
 // Lr / La from the error rate: host code only (vtx_set_donors), in the exact double expressions of the model
 inline Tables make_tables(double e)
 {

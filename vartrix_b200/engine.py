@@ -639,6 +639,39 @@ class Engine:
                     restart_score=arr(out.restart_score, int(restarts), np.int64, (int(restarts),)),
                     restart_iters=arr(out.restart_iters, int(restarts), np.uint32, (int(restarts),)))
 
+    def donors_ambient(self, row, col, ref, alt, n_rows: int, n_cols: int, dosage, error_rate: float = 0.01, rho_permille=None,
+                       grid_batch: int = 0) -> dict:
+        """Donor assignment against ambient RNA (vtx_donors_ambient, include/vartrix_b200.h; DESIGN.md §5h): count entries as
+        cluster_cells takes them and dosage uint8[n_rows, D] as set_donors takes it.  rho_permille=None estimates the ambient
+        fraction; an integer m in 0..500 fixes it at m / 1000 (anything else, e.g. the fraction 0.15, raises).  -> dict of NumPy copies: ll int64[n_cols, H] (x 2^24), counts
+        uint64[n_cols, 3], grid_permille uint16[E], grid_objective int64[E], grid_calls uint64[E, 3] (ascending m),
+        row_alt / row_depth uint64[n_rows], and the scalars rho_permille, rho (= rho_permille / 1000), n_hyp, rows_usable."""
+        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
+        n = len(arrs[0])
+        if any(len(x) != n for x in arrs):
+            raise ValueError("row, col, ref and alt must have the same length")
+        g = np.ascontiguousarray(dosage, dtype=np.uint8)
+        if g.ndim != 2 or g.shape[0] != int(n_rows):
+            raise ValueError(f"dosage must be a [n_rows, donors] array, not shape {g.shape}")
+        if rho_permille is not None and (isinstance(rho_permille, (bool, np.bool_)) or not isinstance(rho_permille, (int, np.integer))):
+            raise TypeError(f"rho_permille must be None or an integer number of thousandths, not {rho_permille!r}")
+        out = _capi.Ambient()
+        p = _capi.AmbientParams(g.shape[1], float(error_rate), -1 if rho_permille is None else int(rho_permille), int(grid_batch))
+        ptr = [x.ctypes.data if n else None for x in arrs]
+        self._ck(self._L.vtx_donors_ambient(self._h, n, *ptr, int(n_rows), int(n_cols), g.ctypes.data if g.size else None,
+                                            C.byref(p), C.byref(out)), "vtx_donors_ambient")
+
+        def arr(ptr, count, dtype, shape):
+            if count == 0:
+                return np.zeros(shape, dtype)
+            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
+        nc, nh, nr, ne = int(out.n_cols), int(out.n_hyp), int(out.n_rows), int(out.n_evaluated)
+        return dict(rho_permille=int(out.rho_permille), rho=int(out.rho_permille) / 1000, n_hyp=nh, rows_usable=int(out.rows_usable),
+                    ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
+                    grid_permille=arr(out.grid_permille, ne, np.uint16, (ne,)), grid_objective=arr(out.grid_objective, ne, np.int64, (ne,)),
+                    grid_calls=arr(out.grid_calls, ne * 3, np.uint64, (ne, 3)), row_alt=arr(out.row_alt, nr, np.uint64, (nr,)),
+                    row_depth=arr(out.row_depth, nr, np.uint64, (nr,)))
+
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()
 
