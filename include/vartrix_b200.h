@@ -447,6 +447,44 @@ int         vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, co
                                const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const uint8_t* dosage,
                                const vtx_ambient_params* params, vtx_ambient* out);
 
+/* ---- genotypes of clusters against ambient RNA, and their match to genotyped samples (the CLI's --out-cluster-genotypes /
+ * --out-cluster-matches; DESIGN.md §5i) ---------------------------------------------------------------------------------------
+ * Over n_rows matrix rows: alt_w / depth_w [row * k + j] and row_used [row] as vtx_cluster_cells returns them (A_kv, T_kv x 2^16,
+ * R_kv = T_kv - A_kv), row_alt / row_depth [row] = A_v, T_v as vtx_donors_ambient returns them (the sums of alt / ref + alt over
+ * every entry at the row).  At rho = m / 1000 a dosage g in {0, 1, 2} expects vtx_donors_ambient's q_vs for q_s = error_rate,
+ * 0.5 and 1 - error_rate, with its int32 logs La_g / Lr_g, and LL_vkg = floor((A_kv La_g + R_kv Lr_g) / 2^16) exactly (int64,
+ * x VTX_DONOR_LL_SCALE).  rho_permille = m fixes rho; -1 estimates it: J(m) = sum over used rows and every cluster of max_g
+ * LL_vkg on vtx_donors_ambient's grid (m = 0, 10, ..., 500, then every m within 9 of the best; the largest J wins, ties the
+ * smallest m).  At the chosen m each (row, cluster) with T_kv > 0 gets GT = argmax_g LL (ties: the lowest g) and
+ * PL_g = floor((10 (LL_max - LL_g) + floor(L10 / 2)) / L10) saturated at 2^31 - 1, L10 = llrint(log(10) 2^24) = 38630967.
+ * GQ = min(99, the second-smallest PL).  With n_samples = S > 0, dosage [row * S + s] is 0, 1, 2 or VTX_GT_MISSING; over the
+ * rows where every sample has a dosage ("compared"), match_ll [j * S + s] = sum of LL_{v,j,g_sv}, match_discordant [j * S + s]
+ * = the compared rows with GQ >= 20 where GT differs from g_sv, match_rows [j] = the compared rows with T_jv > 0 and
+ * match_called [j] = the compared rows with GQ >= 20.
+ *
+ * "Touched" rows are those with T_kv > 0 for some k; gt [t * k + j] (VTX_GT_MISSING where T_jv = 0) and pl [(t * k + j) * 3 + g]
+ * follow `touched` (ascending matrix rows).  rows_fit = used rows that are touched.  Library-owned host memory, valid until the
+ * next vtx_cluster_genotypes or vtx_destroy.  VTX_E_STATE while submits are unfinished; VTX_E_INVALID for k outside 2..32,
+ * n_samples above 1024 (or > 0 with a NULL dosage), error_rate outside [1e-6, 0.25], rho_permille outside -1..500,
+ * alt_w < 0 or > depth_w, depth_w > 2^51, depth_w summing over every row and cluster to more than 2^51 (J and match_ll stay
+ * in int64), row_alt > row_depth or row_depth + 2 reaching 2^53, a dosage other than 0, 1, 2 or VTX_GT_MISSING, or n_rows
+ * reaching 2^32; VTX_E_NOMEM when the device cannot hold about 53 k + 16 bytes per touched row and 4 + S per compared one. */
+typedef struct vtx_cluster_gt_params {
+    uint32_t k; double error_rate; int32_t rho_permille;             /* -1: estimate */
+    uint32_t n_samples;
+} vtx_cluster_gt_params;
+typedef struct vtx_cluster_gt {
+    uint32_t k, n_samples, rho_permille, n_evaluated; uint64_t n_rows, rows_fit, n_touched, rows_compared;
+    const uint16_t* grid_permille; const int64_t* grid_objective;  /* [n_evaluated], ascending m */
+    const uint64_t* touched;                                       /* [n_touched] ascending matrix rows */
+    const uint8_t* gt; const uint32_t* pl;                         /* [n_touched][k], [n_touched][k][3]; VTX_GT_MISSING where T_kv = 0 */
+    const int64_t* match_ll; const uint64_t* match_discordant;     /* [k][n_samples] */
+    const uint64_t* match_rows; const uint64_t* match_called;      /* [k] */
+} vtx_cluster_gt;
+int         vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, const int64_t* depth_w, const uint8_t* row_used,
+                                  const uint64_t* row_alt, const uint64_t* row_depth, const uint8_t* dosage,
+                                  const vtx_cluster_gt_params* params, vtx_cluster_gt* out);
+
 /* Injective code of a cell-barcode tag of the form [ACGT]{1,24}(-N)? with N = 1..99 written without a leading zero:
  * 2 bits per base, 5 bits length, 7 bits N (0 = no suffix); < 2^60.  Returns VTX_NO_CB_KEY if the bytes have another
  * form -- the caller then lists them as an exotic tag (VTX_CB_EXOTIC | i). */

@@ -32,7 +32,7 @@ SYMBOLS = [
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
     "vtx_set_min_base_quality", "vtx_bam_low_base_quality", "vtx_set_locus_stats", "vtx_locus_stats_get",
-    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells", "vtx_donors_ambient",
+    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells", "vtx_donors_ambient", "vtx_cluster_genotypes",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
 CB_EXOTIC = 0x8000000000000000
@@ -130,6 +130,18 @@ class Ambient(C.Structure):        # vtx_ambient
                 ("row_alt", C.POINTER(C.c_uint64)), ("row_depth", C.POINTER(C.c_uint64))]
 
 
+class ClusterGtParams(C.Structure):    # vtx_cluster_gt_params
+    _fields_ = [("k", C.c_uint32), ("error_rate", C.c_double), ("rho_permille", C.c_int32), ("n_samples", C.c_uint32)]
+
+
+class ClusterGt(C.Structure):          # vtx_cluster_gt
+    _fields_ = [("k", C.c_uint32), ("n_samples", C.c_uint32), ("rho_permille", C.c_uint32), ("n_evaluated", C.c_uint32),
+                ("n_rows", C.c_uint64), ("rows_fit", C.c_uint64), ("n_touched", C.c_uint64), ("rows_compared", C.c_uint64),
+                ("grid_permille", C.POINTER(C.c_uint16)), ("grid_objective", C.POINTER(C.c_int64)), ("touched", C.POINTER(C.c_uint64)),
+                ("gt", C.POINTER(C.c_uint8)), ("pl", C.POINTER(C.c_uint32)), ("match_ll", C.POINTER(C.c_int64)),
+                ("match_discordant", C.POINTER(C.c_uint64)), ("match_rows", C.POINTER(C.c_uint64)), ("match_called", C.POINTER(C.c_uint64))]
+
+
 class Metrics(C.Structure):
     _fields_ = [("num_not_cell_bc", C.c_uint64), ("num_non_umi", C.c_uint64), ("num_scored", C.c_uint64)]
 
@@ -219,6 +231,9 @@ def load():
     L.vtx_donors_ambient.restype = C.c_int
     L.vtx_donors_ambient.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                                      C.c_void_p, C.POINTER(AmbientParams), C.POINTER(Ambient)]
+    L.vtx_cluster_genotypes.restype = C.c_int
+    L.vtx_cluster_genotypes.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.POINTER(ClusterGtParams), C.POINTER(ClusterGt)]
     L.vtx_pack_cb.restype = C.c_uint64
     L.vtx_pack_cb.argtypes = [C.c_char_p, C.c_uint32]
     L.vtx_gather_start.restype = C.c_int

@@ -91,6 +91,7 @@ inline bool load_barcodes(const std::string& path, BarcodeList* out, std::string
 struct VcfRecord {
     std::string chrom;
     int64_t pos0 = 0;                     // rec.pos(): 0-based
+    std::string id;                       // the ID column, as written
     std::vector<std::string> alleles;     // REF then ALTs; ALT "." -> only REF (main.rs:654-659)
 };
 
@@ -199,6 +200,7 @@ inline bool read_vcf(const std::string& path, std::vector<VcfRecord>* out, std::
         VcfRecord r;
         r.chrom = f[0];
         r.pos0 = std::strtoll(f[1].c_str(), nullptr, 10) - 1;
+        r.id = f[2];
         r.alleles.push_back(f[3]);
         if (f[4] != ".") {
             size_t a = 0;

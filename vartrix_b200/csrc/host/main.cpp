@@ -27,6 +27,7 @@
 #include "../vtx_donors.cuh"
 #include "../vtx_clusters.cuh"
 #include "../vtx_ambient.cuh"
+#include "../vtx_cluster_gt.cuh"
 
 using namespace vtxhost;
 
@@ -63,6 +64,7 @@ struct Opts {
     uint32_t clusters = 0, cluster_restarts = 8;       // --clusters K, --cluster-restarts R
     uint64_t cluster_seed = 0;                         // --cluster-seed S
     bool cluster_restarts_given = false, cluster_seed_given = false;
+    std::string out_cluster_genotypes, out_cluster_matches;     // --out-cluster-genotypes FILE, --out-cluster-matches FILE
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
     uint32_t min_base_quality = 0;     // --min-base-quality (0: off)
@@ -97,6 +99,10 @@ void usage()
          "      --cluster-restarts R    EM restarts from random starts, the best one is kept, 1 .. 64 [8]\n"
          "      --cluster-seed S        Seed of the restarts' random starts, 0 .. 2^64-1 [0]\n"
          "      --out-cluster-alleles FILE  Per-variant REF / ALT counts of every cluster (TSV, one line per VCF record)\n"
+         "      --out-cluster-genotypes FILE  With --out-clusters: every cluster's genotype at each variant some cell reached (VCF,\n"
+         "                              GT:GQ:PL per cluster), fitted together with the pool's ambient-RNA fraction\n"
+         "      --out-cluster-matches FILE  With --out-clusters: match each cluster's genotypes against the VCF's samples (TSV, one\n"
+         "                              line per cluster: best and second sample, their log-likelihood ratio, discordant calls)\n"
          "  -p, --padding INT           Padding on both sides of the variant [100]\n"
          "  -s, --scoring-method M      consensus | coverage | alt_frac [consensus]\n"
          "      --ref-matrix FILE       Reference matrix (coverage mode) [ref_matrix.mtx]\n"
@@ -200,6 +206,8 @@ bool parse(int argc, char** argv, Opts* o)
         else if (a == "--out-ambient") o->out_ambient = v();
         else if (a == "--out-clusters") o->out_clusters = v();
         else if (a == "--out-cluster-alleles") o->out_cluster_alleles = v();
+        else if (a == "--out-cluster-genotypes") o->out_cluster_genotypes = v();
+        else if (a == "--out-cluster-matches") o->out_cluster_matches = v();
         else if (a == "--clusters" || a == "--cluster-restarts" || a == "--cluster-seed") {
             const std::string t = v();
             char* end = nullptr;
@@ -288,6 +296,14 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --cluster-restarts, --cluster-seed and --out-cluster-alleles only apply with --out-clusters\n");
         return false;
     }
+    if (o->out_clusters.empty() && (!o->out_cluster_genotypes.empty() || !o->out_cluster_matches.empty())) {
+        fprintf(stderr, "error: --out-cluster-genotypes and --out-cluster-matches only apply with --out-clusters\n");
+        return false;
+    }
+    if ((!o->out_cluster_genotypes.empty() || !o->out_cluster_matches.empty()) && !o->dump_staged.empty()) {
+        fprintf(stderr, "error: --out-cluster-genotypes and --out-cluster-matches fit what the GPU run counts: they cannot be combined with --dump-staged\n");
+        return false;
+    }
     if (!o->out_clusters.empty() && !o->dump_staged.empty()) {
         fprintf(stderr, "error: --out-clusters clusters what the GPU run counts: it cannot be combined with --dump-staged\n");
         return false;
@@ -317,6 +333,8 @@ void check_inputs_exist(const Opts& o)
     if (!o.out_ambient.empty()) validate_output_path(o.out_ambient);
     if (!o.out_clusters.empty()) validate_output_path(o.out_clusters);
     if (!o.out_cluster_alleles.empty()) validate_output_path(o.out_cluster_alleles);
+    if (!o.out_cluster_genotypes.empty()) validate_output_path(o.out_cluster_genotypes);
+    if (!o.out_cluster_matches.empty()) validate_output_path(o.out_cluster_matches);
     if (!exists(o.fasta + ".fai")) { LOG_ERR("File %s.fai does not exist", o.fasta.c_str()); exit(1); }
     const size_t dot = o.bam.find_last_of('.');
     const std::string ext = dot == std::string::npos ? "" : o.bam.substr(dot + 1);
@@ -572,6 +590,102 @@ bool write_cluster_alleles(const std::string& path, const std::vector<VcfRecord>
     return fclose(f) == 0;
 }
 
+// --out-cluster-genotypes: VCF 4.2, one record per touched row in row order, GT:GQ:PL per cluster ("./." where no molecule of
+// the cluster reached the row)
+bool write_cluster_genotypes(const std::string& path, const std::vector<VcfRecord>& recs, const vtx_clusters& cl, const vtx_cluster_gt& cg)
+{
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    fprintf(f, "##fileformat=VCFv4.2\n##source=vartrix_b200\n##vartrix_ambient_rna=%.3f\n##vartrix_ambient_rna_estimated=true\n",
+            cg.rho_permille / 1000.0);
+    fputs("##INFO=<ID=USED,Number=0,Type=Flag,Description=\"The cells were clustered and the ambient fraction fitted on this variant\">\n"
+          "##FORMAT=<ID=GT,Number=1,Type=String,Description=\"Genotype\">\n"
+          "##FORMAT=<ID=GQ,Number=1,Type=Integer,Description=\"Genotype quality: the second-smallest PL, at most 99\">\n"
+          "##FORMAT=<ID=PL,Number=G,Type=Integer,Description=\"Phred-scaled genotype likelihoods, with the pool's ambient RNA mixed in\">\n"
+          "#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO\tFORMAT", f);
+    for (uint32_t j = 0; j < cg.k; ++j) fprintf(f, "\tC%u", j);
+    fputc('\n', f);
+    static const char* const kGt[3] = { "0/0", "0/1", "1/1" };
+    for (uint64_t i = 0; i < cg.n_touched; ++i) {
+        const uint64_t v = cg.touched[i];
+        const VcfRecord& r = recs[v];
+        std::string alt;
+        for (size_t a = 1; a < r.alleles.size(); ++a) alt += (a > 1 ? "," : "") + r.alleles[a];
+        fprintf(f, "%s\t%lld\t%s\t%s\t%s\t.\t.\t%s\tGT:GQ:PL", r.chrom.c_str(), (long long)r.pos0 + 1, r.id.c_str(), r.alleles[0].c_str(),
+                alt.empty() ? "." : alt.c_str(), cl.row_used[v] ? "USED" : ".");
+        for (uint32_t j = 0; j < cg.k; ++j) {
+            const uint8_t g = cg.gt[i * cg.k + j];
+            const uint32_t* pl = cg.pl + (i * cg.k + j) * 3;
+            if (g == vtx::cluster_gt::kMissing) fputs("\t./.", f);
+            else fprintf(f, "\t%s:%u:%u,%u,%u", kGt[g], vtx::cluster_gt::gq_of(pl), pl[0], pl[1], pl[2]);
+        }
+        fputc('\n', f);
+    }
+    return fclose(f) == 0;
+}
+
+// --out-cluster-matches: one line per cluster in canonical order; `assigned` gets "C0=S1,C1=.,..."
+bool write_cluster_matches(const std::string& path, const std::vector<std::string>& samples, const vtx_cluster_gt& cg, std::string* assigned)
+{
+    using namespace vtx::cluster_gt;
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    const uint32_t S = cg.n_samples;
+    const double scale = double(vtx::donors::kScale);
+    fputs("cluster\trows\tcalled\tbest_sample\tdiscordant\tsecond_sample\tllr\tassignment", f);
+    for (const std::string& s : samples) fprintf(f, "\tll_%s", s.c_str());
+    fputc('\n', f);
+    for (uint32_t j = 0; j < cg.k; ++j) {
+        const int64_t* M = cg.match_ll + size_t(j) * S;
+        const uint64_t* disc = cg.match_discordant + size_t(j) * S;
+        const Assignment a = assign(M, disc, cg.match_called[j], S);
+        char llr[64] = ".";
+        if (S > 1) snprintf(llr, sizeof(llr), "%.6f", double(a.llr) / scale);
+        const std::string who = a.assigned ? samples[a.best] : ".";
+        fprintf(f, "C%u\t%llu\t%llu\t%s\t%llu\t%s\t%s\t%s", j, (unsigned long long)cg.match_rows[j], (unsigned long long)cg.match_called[j],
+                samples[a.best].c_str(), (unsigned long long)disc[a.best], S > 1 ? samples[a.second].c_str() : ".", llr, who.c_str());
+        for (uint32_t s = 0; s < S; ++s) fprintf(f, "\t%.6f", double(M[s]) / scale);
+        fputc('\n', f);
+        *assigned += (j ? "," : "") + ("C" + std::to_string(j)) + "=" + who;
+    }
+    return fclose(f) == 0;
+}
+
+// --out-cluster-genotypes / --out-cluster-matches: once, on lane 0, after the clustering.  The error rate is §5f's default.
+int cluster_genotypes(const Opts& o, vtx_ctx* ctx, const vtx_result& res, const std::vector<VcfRecord>& recs, const VcfGenotypes& gts,
+                      const vtx_clusters& cl)
+{
+    std::vector<uint64_t> row_alt(recs.size(), 0), row_depth(recs.size(), 0);       // the pool's sums per row
+    for (uint64_t i = 0; i < res.n; ++i) {
+        row_alt[res.row[i]] += res.alt_cnt[i];
+        row_depth[res.row[i]] += uint64_t(res.ref_cnt[i]) + res.alt_cnt[i];
+    }
+    const bool matches = !o.out_cluster_matches.empty();
+    const vtx_cluster_gt_params p{ cl.k, 0.01, -1, matches ? uint32_t(gts.samples.size()) : 0u };
+    vtx_cluster_gt cg{};
+    if (vtx_cluster_genotypes(ctx, recs.size(), cl.alt_w, cl.depth_w, cl.row_used, row_alt.data(), row_depth.data(),
+                              matches ? gts.dosage.data() : nullptr, &p, &cg) != VTX_OK) {
+        printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx));
+        return 1;
+    }
+    int rc = 0;
+    if (!o.out_cluster_genotypes.empty()) {
+        validate_output_path(o.out_cluster_genotypes);
+        if (!write_cluster_genotypes(o.out_cluster_genotypes, recs, cl, cg)) { LOG_ERR("error writing cluster genotype file"); rc = 1; }
+    }
+    std::string assigned;
+    if (matches) {
+        validate_output_path(o.out_cluster_matches);
+        if (!write_cluster_matches(o.out_cluster_matches, gts.samples, cg, &assigned)) { LOG_ERR("error writing cluster match file"); rc = 1; }
+    }
+    uint64_t called = 0;
+    for (uint64_t i = 0; i < cg.n_touched * cg.k; ++i) called += vtx::cluster_gt::gq_of(cg.pl + i * 3) >= vtx::cluster_gt::kMinGq;
+    LOG_INFO("Cluster genotypes: ambient RNA %.3f (estimated, %u fractions evaluated); rows fit: %llu; touched rows: %llu of %zu; genotypes called at GQ >= 20: %llu%s%s",
+             cg.rho_permille / 1000.0, cg.n_evaluated, (unsigned long long)cg.rows_fit, (unsigned long long)cg.n_touched, recs.size(),
+             (unsigned long long)called, matches ? "; assignments: " : "", assigned.c_str());
+    return rc;
+}
+
 }  // namespace
 
 // One GPU of the run: its own engine context, a contiguous range of shards, a thread that feeds it in order.
@@ -619,15 +733,23 @@ int main(int argc, char** argv)
     if (!load_barcodes(o.barcodes, &bcs, &err)) { LOG_ERR("%s", err.c_str()); return 1; }
     LOG_INFO("Loaded %zu barcodes", bcs.keys.size());
 
-    // --out-donors: the VCF (with its sample columns) is read before any GPU work, so that a bad donor list is refused first
+    // --out-donors / --out-cluster-matches: the VCF (with its sample columns) is read once, before any GPU work, so that a bad
+    // donor list or sample header is refused first
     std::vector<VcfRecord> recs;
     const bool with_donors = !o.out_donors.empty();
     const bool with_ambient = !o.ambient_rna.empty();      // the donors are scored once, after the finish, over the result
+    const bool with_matches = !o.out_cluster_matches.empty();
+    const bool with_cluster_gt = with_matches || !o.out_cluster_genotypes.empty();
     DonorTable donors;
-    if (with_donors) {
-        VcfGenotypes gts;
+    VcfGenotypes gts;
+    if (with_donors || with_matches) {
         if (!read_vcf(o.vcf, &recs, &err, &gts)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
-        if (!select_donors(o.donors, gts, recs, &donors, &err)) { fprintf(stderr, "error: %s\n", err.c_str()); return 1; }
+        if (with_donors && !select_donors(o.donors, gts, recs, &donors, &err)) { fprintf(stderr, "error: %s\n", err.c_str()); return 1; }
+        if (with_matches && (gts.samples.empty() || gts.samples.size() > vtx::cluster_gt::kMaxSamples)) {
+            fprintf(stderr, "error: --out-cluster-matches needs 1 to %u sample columns in the VCF, not %zu\n", vtx::cluster_gt::kMaxSamples,
+                    gts.samples.size());
+            return 1;
+        }
     }
 
     // CUDA context creation takes ~1 s per device: start it now, in the background, while the VCF is parsed and the
@@ -664,7 +786,7 @@ int main(int argc, char** argv)
         }
     }
 
-    if (!with_donors && !read_vcf(o.vcf, &recs, &err)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
+    if (!with_donors && !with_matches && !read_vcf(o.vcf, &recs, &err)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
     if (recs.empty()) LOG_ERR("Warning! Zero variants found in input VCF. Output matrices will be by definition empty but will still be generated.");
     LOG_INFO("Initialized a %zu variants x %zu cell barcodes matrix", recs.size(), bcs.keys.size());
     LOG_INFO("[%.3f s] inputs parsed", now_s());
@@ -1082,6 +1204,7 @@ int main(int argc, char** argv)
             LOG_INFO("Clusters: %u, restarts %u, seed %llu; best restart %u after %u iterations; rows used: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
                      cl.k, o.cluster_restarts, (unsigned long long)o.cluster_seed, cl.best_restart, cl.restart_iters[cl.best_restart],
                      (unsigned long long)cl.rows_used, recs.size(), (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
+            if (with_cluster_gt && cluster_genotypes(o, ctx, res, recs, gts, cl) != 0) rc = 1;
         }
     }
     LOG_INFO("[%.3f s] outputs written", now_s());

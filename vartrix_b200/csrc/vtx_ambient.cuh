@@ -55,6 +55,13 @@ inline Fractions fractions(double e)
     return f;
 }
 
+// log_fixed of (1 - rho) q + rho f: La_vs with q = q_s, f = f_v; Lr_vs with their complements
+VTX_AM_HD inline int32_t mix_log(double q, double rho, double orho, double f)
+{
+    using namespace clusters;
+    return log_fixed(d_add(d_mul(orho, q), d_mul(rho, f)));
+}
+
 // the tables of one row at m: out[2 s] = La_vs, out[2 s + 1] = Lr_vs
 VTX_AM_HD inline void row_logs(const Fractions& fr, uint32_t m, uint64_t A, uint64_t T, int32_t* out)
 {
@@ -63,9 +70,18 @@ VTX_AM_HD inline void row_logs(const Fractions& fr, uint32_t m, uint64_t A, uint
     const double f = d_div(double(A + 1), den), of = d_div(double(T - A + 1), den);
     const double rho = d_div(double(m), 1000.0), orho = d_div(double(1000 - m), 1000.0);
     for (int s = 0; s < 5; ++s) {
-        out[2 * s] = log_fixed(d_add(d_mul(orho, fr.q[s]), d_mul(rho, f)));
-        out[2 * s + 1] = log_fixed(d_add(d_mul(orho, fr.oq[s]), d_mul(rho, of)));
+        out[2 * s] = mix_log(fr.q[s], rho, orho, f);
+        out[2 * s + 1] = mix_log(fr.oq[s], rho, orho, of);
     }
+}
+
+// one entry of row_logs: La_vs (alt) or Lr_vs
+VTX_AM_HD inline int32_t row_log(const Fractions& fr, uint32_t m, uint64_t A, uint64_t T, int s, bool alt)
+{
+    using namespace clusters;
+    const double den = double(T + 2);
+    const double f = alt ? d_div(double(A + 1), den) : d_div(double(T - A + 1), den);
+    return mix_log(alt ? fr.q[s] : fr.oq[s], d_div(double(m), 1000.0), d_div(double(1000 - m), 1000.0), f);
 }
 
 // ---- serial body (tests/ambient_shim.cpp): vtx_k_am_score computes the same integers with one lane per hypothesis ----------

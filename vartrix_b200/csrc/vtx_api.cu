@@ -10,6 +10,7 @@
 #include "vtx_donors.cuh"
 #include "vtx_clusters.cuh"
 #include "vtx_ambient.cuh"
+#include "vtx_cluster_gt.cuh"
 
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
@@ -163,6 +164,13 @@ struct vtx_ctx {
     std::vector<int64_t> h_am_ll, h_am_obj;
     std::vector<uint64_t> h_am_cnt, h_am_calls, h_am_alt, h_am_depth;
     std::vector<uint16_t> h_am_m;
+    // vtx_cluster_genotypes: device work buffers and the host outputs of the last call
+    DBuf cg_AT, cg_rows, cg_fit, cg_ll, cg_gt, cg_pl, cg_cmp, cg_dos, cg_acc;
+    std::vector<int64_t> h_cg_obj, h_cg_M;
+    std::vector<uint64_t> h_cg_touched, h_cg_acc;
+    std::vector<uint16_t> h_cg_m;
+    std::vector<uint8_t> h_cg_gt;
+    std::vector<uint32_t> h_cg_pl;
     HostBuf h_stage;                                  // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
@@ -1103,6 +1111,32 @@ int validate_entries(vtx_ctx* ctx, const char* fn, uint64_t n, const uint32_t* r
     return VTX_OK;
 }
 
+// §5h's estimate of m: the coarse grid, then every m within kFineReach of its winner; the largest J wins, ties the smallest m.
+// evaluate(list) appends J of every m in `list` to obj and returns a VTX code; ms / obj end with every evaluated m in that order.
+template <typename Evaluate>
+int estimate_permille(std::vector<uint16_t>& ms, std::vector<int64_t>& obj, Evaluate evaluate, uint32_t* chosen)
+{
+    using namespace ambient;
+    auto best_of = [&]() {
+        size_t w = 0;
+        for (size_t i = 1; i < ms.size(); ++i)
+            if (obj[i] > obj[w] || (obj[i] == obj[w] && ms[i] < ms[w])) w = i;
+        return ms[w];
+    };
+    for (uint32_t m = 0; m <= uint32_t(kMaxPermille); m += kCoarseStep) ms.push_back(uint16_t(m));
+    int rc = evaluate(ms);
+    if (rc) return rc;
+    const uint32_t mc = best_of();
+    std::vector<uint16_t> fine;
+    for (uint32_t m = mc > kFineReach ? mc - kFineReach : 0; m <= std::min<uint32_t>(kMaxPermille, mc + kFineReach); ++m)
+        if (m % kCoarseStep) fine.push_back(uint16_t(m));
+    rc = evaluate(fine);
+    if (rc) return rc;
+    ms.insert(ms.end(), fine.begin(), fine.end());
+    *chosen = best_of();
+    return VTX_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -1938,29 +1972,13 @@ int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
         }
         return VTX_OK;
     };
-    // the estimate: the coarse grid, then every m within kFineReach of its winner; the largest J wins, ties the smallest m
     std::vector<uint16_t> ms;
     std::vector<int64_t> obj;
     std::vector<uint64_t> calls;
-    auto best_of = [&]() {
-        size_t w = 0;
-        for (size_t i = 1; i < ms.size(); ++i)
-            if (obj[i] > obj[w] || (obj[i] == obj[w] && ms[i] < ms[w])) w = i;
-        return ms[w];
-    };
     uint32_t chosen = uint32_t(given);
     if (given < 0) {
-        for (uint32_t m = 0; m <= uint32_t(kMaxPermille); m += kCoarseStep) ms.push_back(uint16_t(m));
-        rc = evaluate(ms, false, &obj, &calls);
+        rc = estimate_permille(ms, obj, [&](const std::vector<uint16_t>& list) { return evaluate(list, false, &obj, &calls); }, &chosen);
         if (rc) return rc;
-        const uint32_t mc = best_of();
-        std::vector<uint16_t> fine;
-        for (uint32_t m = mc > kFineReach ? mc - kFineReach : 0; m <= std::min<uint32_t>(kMaxPermille, mc + kFineReach); ++m)
-            if (m % kCoarseStep) fine.push_back(uint16_t(m));
-        rc = evaluate(fine, false, &obj, &calls);
-        if (rc) return rc;
-        ms.insert(ms.end(), fine.begin(), fine.end());
-        chosen = best_of();
     }
     std::vector<int64_t> obj_f;
     std::vector<uint64_t> calls_f;
@@ -1996,6 +2014,192 @@ int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     out->ll = ctx->h_am_ll.data(); out->counts = ctx->h_am_cnt.data();
     out->grid_permille = ctx->h_am_m.data(); out->grid_objective = ctx->h_am_obj.data(); out->grid_calls = ctx->h_am_calls.data();
     out->row_alt = ctx->h_am_alt.data(); out->row_depth = ctx->h_am_depth.data();
+    return VTX_OK;
+}
+
+int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, const int64_t* depth_w, const uint8_t* row_used,
+                          const uint64_t* row_alt, const uint64_t* row_depth, const uint8_t* dosage,
+                          const vtx_cluster_gt_params* params, vtx_cluster_gt* out)
+{
+    using namespace cluster_gt;
+    if (!ctx || !params || !out) return VTX_E_INVALID;
+    *out = vtx_cluster_gt{};
+    if (!ctx->finished || ctx->gather_pending)
+        return set_err(ctx, VTX_E_STATE, "vtx_cluster_genotypes: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const uint32_t K = params->k, S = params->n_samples;
+    const int32_t given = params->rho_permille;
+    if (K < clusters::kMinK || K > clusters::kMaxK)
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: k = %u; 2 to 32 clusters are supported", K);
+    if (S > kMaxSamples) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: %u samples; 0 to 1024 are supported", S);
+    if (S && !dosage) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: dosage is NULL");
+    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: error rate %g outside [1e-6, 0.25]", params->error_rate);
+    if (given < -1 || given > ambient::kMaxPermille)
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: rho_permille %d; -1 (estimate) or 0 to 500", given);
+    if (n_rows && (!alt_w || !depth_w || !row_used || !row_alt || !row_depth))
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: a row array is NULL");
+    if (n_rows > 0xFFFFFFFFull)
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: %llu rows; must be below 2^32", (unsigned long long)n_rows);
+
+    // validate in one pass, and list the touched rows (T_kv > 0 for some k), the fitted ones (used and touched) and the compared
+    // ones (touched, every sample has a dosage)
+    std::vector<uint32_t> touched, fit, cmp;
+    uint64_t total = 0, rows_compared = 0;
+    for (uint64_t v = 0; v < n_rows; ++v) {
+        bool reached = false;
+        for (uint32_t k = 0; k < K; ++k) {
+            const int64_t a = alt_w[v * K + k], t = depth_w[v * K + k];
+            if (a < 0 || a > t || t > kMaxDepthW)
+                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: row %llu, cluster %u: alt_w %lld, depth_w %lld (0 <= alt_w <= depth_w <= 2^51)",
+                               (unsigned long long)v, k, (long long)a, (long long)t);
+            total += uint64_t(t);
+            if (total > kMaxTotalDepthW)
+                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: depth_w sums to more than 2^51 over the rows; the fit's int64 sums would not be exact");
+            reached = reached || t > 0;
+        }
+        if (row_alt[v] > row_depth[v] || row_depth[v] > ambient::kMaxRowDepth)
+            return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: row %llu: row_alt %llu, row_depth %llu (row_alt <= row_depth < 2^53 - 2)",
+                           (unsigned long long)v, (unsigned long long)row_alt[v], (unsigned long long)row_depth[v]);
+        bool all = S > 0;
+        for (uint32_t s = 0; s < S; ++s) {
+            const uint8_t g = dosage[v * S + s];
+            if (g > 2 && g != kMissing)
+                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: dosage %u at row %llu, sample %u (0, 1, 2 or VTX_GT_MISSING)",
+                               unsigned(g), (unsigned long long)v, s);
+            all = all && g != kMissing;
+        }
+        rows_compared += all;
+        if (!reached) continue;
+        if (row_used[v]) fit.push_back(uint32_t(touched.size()));
+        if (all) cmp.push_back(uint32_t(touched.size()));
+        touched.push_back(uint32_t(v));
+    }
+    const uint32_t n_t = uint32_t(touched.size()), n_fit = uint32_t(fit.size()), n_cmp = uint32_t(cmp.size());
+    {   // every buffer is allocated with 1/8 to spare (ensure)
+        const double need = (double(n_t) * (53.0 * K + 16) + double(n_fit) * 4 + double(n_cmp) * (4.0 + S) + 16.0 * K * (S + 1) + 4096) * 1.125;
+        CK(cudaSetDevice(ctx->device));
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        size_t held = 0;
+        for (DBuf* b : { &ctx->cg_AT, &ctx->cg_rows, &ctx->cg_fit, &ctx->cg_ll, &ctx->cg_gt, &ctx->cg_pl, &ctx->cg_cmp, &ctx->cg_dos, &ctx->cg_acc })
+            held += b->cap;
+        if (need > double(free_b) + double(held))
+            return set_err(ctx, VTX_E_NOMEM, "vtx_cluster_genotypes needs %.0f MB of device memory, %.0f MB are free", need * 1e-6,
+                           (double(free_b) + double(held)) * 1e-6);
+    }
+    // the touched rows' inputs, compacted: A, T [touched][K], then A_v, T_v [touched]; the compared rows' dosages
+    std::vector<int64_t> at(size_t(n_t) * K * 2);
+    std::vector<uint64_t> rows(size_t(n_t) * 2);
+    for (uint32_t i = 0; i < n_t; ++i) {
+        const size_t v = touched[i];
+        memcpy(at.data() + size_t(i) * K, alt_w + v * K, size_t(K) * 8);
+        memcpy(at.data() + (size_t(n_t) + i) * K, depth_w + v * K, size_t(K) * 8);
+        rows[i] = row_alt[v];
+        rows[n_t + i] = row_depth[v];
+    }
+    std::vector<uint8_t> dos(size_t(n_cmp) * S);
+    for (uint32_t i = 0; i < n_cmp; ++i) memcpy(dos.data() + size_t(i) * S, dosage + size_t(touched[cmp[i]]) * S, S);
+
+    cudaStream_t st = ctx->stream;
+    ENS(ctx->cg_AT, at.size() * 8 + 8);
+    ENS(ctx->cg_rows, rows.size() * 8 + 8);
+    ENS(ctx->cg_fit, size_t(n_fit) * 4 + 4);
+    ENS(ctx->cg_ll, size_t(n_t) * K * 24 + 8);
+    ENS(ctx->cg_gt, size_t(n_t) * K + 8);
+    ENS(ctx->cg_pl, size_t(n_t) * K * 12 + 8);
+    ENS(ctx->cg_cmp, size_t(n_cmp) * 4 + 4);
+    ENS(ctx->cg_dos, dos.size() + 8);
+    ENS(ctx->cg_acc, (size_t(ambient::kMaxBatch) + 2 * size_t(K) * S + 2 * K) * 8);
+    if (n_t) {
+        CK(cudaMemcpyAsync(ctx->cg_AT.p, at.data(), at.size() * 8, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cg_rows.p, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, st));
+    }
+    if (n_fit) CK(cudaMemcpyAsync(ctx->cg_fit.p, fit.data(), size_t(n_fit) * 4, cudaMemcpyHostToDevice, st));
+    if (n_cmp) {
+        CK(cudaMemcpyAsync(ctx->cg_cmp.p, cmp.data(), size_t(n_cmp) * 4, cudaMemcpyHostToDevice, st));
+        if (S) CK(cudaMemcpyAsync(ctx->cg_dos.p, dos.data(), dos.size(), cudaMemcpyHostToDevice, st));
+    }
+    const int64_t* d_A = P<int64_t>(ctx->cg_AT);
+    const int64_t* d_T = d_A + size_t(n_t) * K;
+    const unsigned long long* d_rowA = P<unsigned long long>(ctx->cg_rows);
+    const unsigned long long* d_rowT = d_rowA + n_t;
+    unsigned long long* d_J = P<unsigned long long>(ctx->cg_acc);
+    const ambient::Fractions fr = ambient::fractions(params->error_rate);
+
+    // J(m) of every m in the list, one launch per batch of up to kMaxBatch
+    std::vector<uint16_t> ms;
+    std::vector<int64_t> obj;
+    std::vector<unsigned long long> h_J(ambient::kMaxBatch);
+    auto evaluate = [&](const std::vector<uint16_t>& list) -> int {
+        for (size_t o = 0; o < list.size(); o += ambient::kMaxBatch) {
+            ambient::Batch bt{};
+            bt.n = uint32_t(std::min<size_t>(ambient::kMaxBatch, list.size() - o));
+            for (uint32_t b = 0; b < bt.n; ++b) bt.m[b] = list[o + b];
+            CK(cudaMemsetAsync(d_J, 0, size_t(ambient::kMaxBatch) * 8, st));
+            if (n_fit) {
+                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_fit * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
+                vtx_k_cg_fit<<<g, kCgThreads, 0, st>>>(bt, fr, K, n_fit, P<uint32_t>(ctx->cg_fit), d_rowA, d_rowT, d_A, d_T, d_J);
+                CK(cudaGetLastError());
+            }
+            CK(cudaMemcpyAsync(h_J.data(), d_J, size_t(bt.n) * 8, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            for (uint32_t b = 0; b < bt.n; ++b) obj.push_back(int64_t(h_J[b]));
+        }
+        return VTX_OK;
+    };
+    uint32_t chosen = uint32_t(given);
+    int rc = VTX_OK;
+    if (given < 0) rc = estimate_permille(ms, obj, evaluate, &chosen);
+    else { ms.assign(1, uint16_t(chosen)); rc = evaluate(ms); }
+    if (rc) return rc;
+
+    // the calls at the chosen m, then the match
+    if (n_t) {
+        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_t) * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
+        vtx_k_cg_call<<<g, kCgThreads, 0, st>>>(chosen, fr, K, n_t, d_rowA, d_rowT, d_A, d_T, P<int64_t>(ctx->cg_ll), P<uint8_t>(ctx->cg_gt),
+                                                 P<uint32_t>(ctx->cg_pl));
+        CK(cudaGetLastError());
+    }
+    unsigned long long* d_M = d_J + ambient::kMaxBatch;
+    const size_t n_acc = 2 * size_t(K) * S + 2 * K;                   // M, discordant [K][S], then rows, called [K]
+    CK(cudaMemsetAsync(d_M, 0, n_acc * 8, st));
+    if (S && n_cmp) {
+        const uint32_t ys = (S + kMatchSamples - 1) / kMatchSamples;
+        // about four CTAs per SM in all, each over whole tiles of rows
+        const uint64_t xs_want = std::max<uint64_t>(1, uint64_t(ctx->n_sm) * 4 / ys);
+        const uint64_t tiles = (n_cmp + kMatchRows - 1) / kMatchRows;
+        const uint32_t rows_per_cta = uint32_t((tiles + xs_want - 1) / xs_want) * kMatchRows;
+        const uint32_t xs = uint32_t((n_cmp + rows_per_cta - 1) / rows_per_cta);
+        vtx_k_cg_match<<<dim3(xs, ys), kCgThreads, 0, st>>>(K, S, n_cmp, rows_per_cta, P<uint32_t>(ctx->cg_cmp), P<uint8_t>(ctx->cg_dos),
+                                                             P<int64_t>(ctx->cg_ll), P<uint8_t>(ctx->cg_gt), P<uint32_t>(ctx->cg_pl), d_M,
+                                                             d_M + size_t(K) * S, d_M + 2 * size_t(K) * S, d_M + 2 * size_t(K) * S + K);
+        CK(cudaGetLastError());
+    }
+    ctx->h_cg_gt.resize(size_t(n_t) * K);
+    ctx->h_cg_pl.resize(size_t(n_t) * K * 3);
+    ctx->h_cg_acc.resize(n_acc);
+    if (n_t) {
+        CK(cudaMemcpyAsync(ctx->h_cg_gt.data(), ctx->cg_gt.p, ctx->h_cg_gt.size(), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_cg_pl.data(), ctx->cg_pl.p, ctx->h_cg_pl.size() * 4, cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaMemcpyAsync(ctx->h_cg_acc.data(), d_M, n_acc * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+
+    std::vector<size_t> order(ms.size());
+    for (size_t i = 0; i < order.size(); ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](size_t x, size_t y) { return ms[x] < ms[y]; });
+    ctx->h_cg_m.resize(ms.size()); ctx->h_cg_obj.resize(ms.size());
+    for (size_t i = 0; i < order.size(); ++i) { ctx->h_cg_m[i] = ms[order[i]]; ctx->h_cg_obj[i] = obj[order[i]]; }
+    ctx->h_cg_touched.assign(touched.begin(), touched.end());
+    ctx->h_cg_M.resize(size_t(K) * S);
+    for (size_t i = 0; i < ctx->h_cg_M.size(); ++i) ctx->h_cg_M[i] = int64_t(ctx->h_cg_acc[i]);
+
+    out->k = K; out->n_samples = S; out->rho_permille = chosen; out->n_evaluated = uint32_t(ms.size());
+    out->n_rows = n_rows; out->rows_fit = n_fit; out->n_touched = n_t; out->rows_compared = rows_compared;
+    out->grid_permille = ctx->h_cg_m.data(); out->grid_objective = ctx->h_cg_obj.data();
+    out->touched = ctx->h_cg_touched.data(); out->gt = ctx->h_cg_gt.data(); out->pl = ctx->h_cg_pl.data();
+    out->match_ll = ctx->h_cg_M.data(); out->match_discordant = ctx->h_cg_acc.data() + size_t(K) * S;
+    out->match_rows = ctx->h_cg_acc.data() + 2 * size_t(K) * S; out->match_called = out->match_rows + K;
     return VTX_OK;
 }
 

@@ -672,6 +672,51 @@ class Engine:
                     grid_calls=arr(out.grid_calls, ne * 3, np.uint64, (ne, 3)), row_alt=arr(out.row_alt, nr, np.uint64, (nr,)),
                     row_depth=arr(out.row_depth, nr, np.uint64, (nr,)))
 
+    def cluster_genotypes(self, clusters: dict, row_alt, row_depth, dosage=None, error_rate: float = 0.01, rho_permille=None) -> dict:
+        """Genotypes of the clusters against ambient RNA and their match to genotyped samples (vtx_cluster_genotypes,
+        include/vartrix_b200.h; DESIGN.md §5i): `clusters` is the dict cluster_cells returns, row_alt / row_depth the pool's
+        ALT and REF + ALT sums per row (uint64[n_rows], as donors_ambient returns them), dosage None or uint8[n_rows, S] as
+        set_donors takes it.  rho_permille=None estimates the ambient fraction; an integer m in 0..500 fixes it at m / 1000.
+        -> dict of NumPy copies: grid_permille uint16[E], grid_objective int64[E] (ascending m), touched uint64[n_touched],
+        gt uint8[n_touched, k] (GT_MISSING where no molecule reached the cluster), pl uint32[n_touched, k, 3], match_ll
+        int64[k, S] (x 2^24), match_discordant uint64[k, S], match_rows / match_called uint64[k], and the scalars rho_permille,
+        rho, rows_fit, rows_compared."""
+        A = np.ascontiguousarray(clusters["alt_w"], dtype=np.int64)
+        T = np.ascontiguousarray(clusters["depth_w"], dtype=np.int64)
+        used = np.ascontiguousarray(clusters["row_used"], dtype=np.uint8)
+        if A.ndim != 2 or A.shape != T.shape or used.shape != (A.shape[0],):
+            raise ValueError("clusters must hold alt_w / depth_w [n_rows, k] and row_used [n_rows]")
+        n_rows, k = A.shape
+        ra = np.ascontiguousarray(row_alt, dtype=np.uint64)
+        rd = np.ascontiguousarray(row_depth, dtype=np.uint64)
+        if ra.shape != (n_rows,) or rd.shape != (n_rows,):
+            raise ValueError(f"row_alt and row_depth must have {n_rows} entries")
+        g = None
+        if dosage is not None:
+            g = np.ascontiguousarray(dosage, dtype=np.uint8)
+            if g.ndim != 2 or g.shape[0] != n_rows:
+                raise ValueError(f"dosage must be a [n_rows, samples] array, not shape {g.shape}")
+        s = 0 if g is None else g.shape[1]
+        if rho_permille is not None and (isinstance(rho_permille, (bool, np.bool_)) or not isinstance(rho_permille, (int, np.integer))):
+            raise TypeError(f"rho_permille must be None or an integer number of thousandths, not {rho_permille!r}")
+        out = _capi.ClusterGt()
+        p = _capi.ClusterGtParams(k, float(error_rate), -1 if rho_permille is None else int(rho_permille), s)
+        ptr = [x.ctypes.data if n_rows else None for x in (A, T, used, ra, rd)]
+        self._ck(self._L.vtx_cluster_genotypes(self._h, n_rows, *ptr, g.ctypes.data if g is not None and g.size else None,
+                                               C.byref(p), C.byref(out)), "vtx_cluster_genotypes")
+
+        def arr(ptr, count, dtype, shape):
+            if count == 0:
+                return np.zeros(shape, dtype)
+            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
+        ne, nt = int(out.n_evaluated), int(out.n_touched)
+        return dict(rho_permille=int(out.rho_permille), rho=int(out.rho_permille) / 1000, rows_fit=int(out.rows_fit),
+                    rows_compared=int(out.rows_compared), grid_permille=arr(out.grid_permille, ne, np.uint16, (ne,)),
+                    grid_objective=arr(out.grid_objective, ne, np.int64, (ne,)), touched=arr(out.touched, nt, np.uint64, (nt,)),
+                    gt=arr(out.gt, nt * k, np.uint8, (nt, k)), pl=arr(out.pl, nt * k * 3, np.uint32, (nt, k, 3)),
+                    match_ll=arr(out.match_ll, k * s, np.int64, (k, s)), match_discordant=arr(out.match_discordant, k * s, np.uint64, (k, s)),
+                    match_rows=arr(out.match_rows, k, np.uint64, (k,)), match_called=arr(out.match_called, k, np.uint64, (k,)))
+
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()
 
