@@ -472,6 +472,11 @@ class Engine:
     def sync(self):
         self._ck(self._L.vtx_sync(self._h), "vtx_sync")
 
+    def wait_copies(self):
+        """Wait until the host->device copies of every submit so far have landed (vtx_wait_copies): the host arrays of
+        those submits may then be overwritten, though their kernels may still be running."""
+        self._ck(self._L.vtx_wait_copies(self._h), "vtx_wait_copies")
+
     def timing(self) -> dict:
         t = _capi.Timing()
         self._ck(self._L.vtx_last_timing(self._h, C.byref(t)), "vtx_last_timing")
