@@ -485,6 +485,43 @@ int         vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* 
                                   const uint64_t* row_alt, const uint64_t* row_depth, const uint8_t* dosage,
                                   const vtx_cluster_gt_params* params, vtx_cluster_gt* out);
 
+/* ---- cells called against their clusters' fitted genotypes and ambient RNA, with the clusters refit from their singlets (the
+ * CLI's --out-cluster-calls; DESIGN.md §5j) -------------------------------------------------------------------------------------
+ * Count entries (row, col, ref_cnt, alt_cnt) as vtx_cluster_cells takes them, and that call's k, alt_w / depth_w [row * k + j] and
+ * row_used [row].  Round 0 fits vtx_cluster_genotypes' model (rho estimated, error_rate as there) on alt_w / depth_w; every later
+ * round first rebuilds the sums from the previous round's labels: A_kv = 2^16 sum a, T_kv = 2^16 sum (r + a) over the entries of
+ * the cells labelled k.  At the round's m a (touched row, cluster) has code GT when GQ >= 20, else P (no called genotype); a row
+ * with a called code is scored.  A hypothesis (i, j) in vtx_set_donors' order expects vtx_donors_ambient's q_vs for s = g_i + g_j
+ * when both are called, (1 - rho)((q_2g + f_v) / 2) + rho f_v when one is (g its GT), f_v when neither is; cells add r Lr + a La
+ * (int32 logs, x VTX_DONOR_LL_SCALE) at scored rows and are called with T = 5 nats.  A singlet on k is labelled k, every other
+ * cell VTX_NO_LABEL.  The loop stops when a round's labels equal the previous round's (converged = 1) or after max_rounds rounds
+ * after round 0 (converged = 0; max_rounds = 0 runs round 0 only).
+ *
+ * out->ll [c * n_hyp + h] and counts [c * 3 + {scored rows, ref, alt}] are the last round's, as vtx_donor_ll_get returns them;
+ * label [c] its labels; rounds [r] per round; touched / gt / pl the last round's fit as vtx_cluster_genotypes returns them.
+ * Library-owned host memory, valid until the next vtx_cluster_refine or vtx_destroy.  VTX_E_STATE while submits are unfinished;
+ * VTX_E_INVALID for k outside 2..32, error_rate outside [1e-6, 0.25], max_rounds above 32, a bad entry (as vtx_cluster_cells),
+ * 2^16 x the entries' ref + alt summing to more than 2^51, or alt_w / depth_w outside vtx_cluster_genotypes' bounds;
+ * VTX_E_NOMEM when the device cannot hold 28 bytes per entry, about 70 k + 150 bytes per row and 4 k + 8 n_hyp + 40 per cell. */
+#define VTX_NO_LABEL 0xFFFFFFFFu
+typedef struct vtx_cluster_calls_params { uint32_t k; double error_rate; uint32_t max_rounds; } vtx_cluster_calls_params;
+typedef struct vtx_cluster_calls_round {
+    uint32_t rho_permille, reserved; uint64_t rows_fit, n_touched, rows_scored;
+    uint64_t calls[3];                /* singlet, doublet, unassigned */
+    uint64_t changed;                 /* labels that differ from the previous round's (round 0: from VTX_NO_LABEL) */
+} vtx_cluster_calls_round;
+typedef struct vtx_cluster_calls {
+    uint32_t k, n_cols, n_hyp, n_rounds; int32_t converged; uint32_t reserved; uint64_t n_rows, n_touched;
+    const int64_t* ll; const uint64_t* counts;       /* [n_cols][n_hyp] x 2^24, [n_cols][3] */
+    const uint32_t* label;                           /* [n_cols] cluster or VTX_NO_LABEL */
+    const vtx_cluster_calls_round* rounds;          /* [n_rounds] */
+    const uint64_t* touched;                         /* [n_touched] ascending matrix rows */
+    const uint8_t* gt; const uint32_t* pl;           /* [n_touched][k], [n_touched][k][3] */
+} vtx_cluster_calls;
+int         vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                               const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const int64_t* alt_w, const int64_t* depth_w,
+                               const uint8_t* row_used, const vtx_cluster_calls_params* params, vtx_cluster_calls* out);
+
 /* Injective code of a cell-barcode tag of the form [ACGT]{1,24}(-N)? with N = 1..99 written without a leading zero:
  * 2 bits per base, 5 bits length, 7 bits N (0 = no suffix); < 2^60.  Returns VTX_NO_CB_KEY if the bytes have another
  * form -- the caller then lists them as an exotic tag (VTX_CB_EXOTIC | i). */

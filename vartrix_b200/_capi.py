@@ -32,9 +32,10 @@ SYMBOLS = [
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
     "vtx_set_min_base_quality", "vtx_bam_low_base_quality", "vtx_set_locus_stats", "vtx_locus_stats_get",
-    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells", "vtx_donors_ambient", "vtx_cluster_genotypes",
+    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells", "vtx_donors_ambient", "vtx_cluster_genotypes", "vtx_cluster_refine",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
+NO_LABEL = 0xFFFFFFFF     # VTX_NO_LABEL: a cell vtx_cluster_refine did not call singlet
 CB_EXOTIC = 0x8000000000000000
 GATHER_ALL = -1
 BAND_FULL, BAND_MODEL = 0, 1
@@ -142,6 +143,22 @@ class ClusterGt(C.Structure):          # vtx_cluster_gt
                 ("match_discordant", C.POINTER(C.c_uint64)), ("match_rows", C.POINTER(C.c_uint64)), ("match_called", C.POINTER(C.c_uint64))]
 
 
+class ClusterCallsParams(C.Structure):     # vtx_cluster_calls_params
+    _fields_ = [("k", C.c_uint32), ("error_rate", C.c_double), ("max_rounds", C.c_uint32)]
+
+
+class ClusterCallsRound(C.Structure):      # vtx_cluster_calls_round
+    _fields_ = [("rho_permille", C.c_uint32), ("reserved", C.c_uint32), ("rows_fit", C.c_uint64), ("n_touched", C.c_uint64),
+                ("rows_scored", C.c_uint64), ("calls", C.c_uint64 * 3), ("changed", C.c_uint64)]
+
+
+class ClusterCalls(C.Structure):           # vtx_cluster_calls
+    _fields_ = [("k", C.c_uint32), ("n_cols", C.c_uint32), ("n_hyp", C.c_uint32), ("n_rounds", C.c_uint32), ("converged", C.c_int32),
+                ("reserved", C.c_uint32), ("n_rows", C.c_uint64), ("n_touched", C.c_uint64), ("ll", C.POINTER(C.c_int64)),
+                ("counts", C.POINTER(C.c_uint64)), ("label", C.POINTER(C.c_uint32)), ("rounds", C.POINTER(ClusterCallsRound)),
+                ("touched", C.POINTER(C.c_uint64)), ("gt", C.POINTER(C.c_uint8)), ("pl", C.POINTER(C.c_uint32))]
+
+
 class Metrics(C.Structure):
     _fields_ = [("num_not_cell_bc", C.c_uint64), ("num_non_umi", C.c_uint64), ("num_scored", C.c_uint64)]
 
@@ -234,6 +251,9 @@ def load():
     L.vtx_cluster_genotypes.restype = C.c_int
     L.vtx_cluster_genotypes.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.POINTER(ClusterGtParams), C.POINTER(ClusterGt)]
+    L.vtx_cluster_refine.restype = C.c_int
+    L.vtx_cluster_refine.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ClusterCallsParams), C.POINTER(ClusterCalls)]
     L.vtx_pack_cb.restype = C.c_uint64
     L.vtx_pack_cb.argtypes = [C.c_char_p, C.c_uint32]
     L.vtx_gather_start.restype = C.c_int

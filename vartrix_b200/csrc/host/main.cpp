@@ -28,6 +28,7 @@
 #include "../vtx_clusters.cuh"
 #include "../vtx_ambient.cuh"
 #include "../vtx_cluster_gt.cuh"
+#include "../vtx_cluster_refine.cuh"
 
 using namespace vtxhost;
 
@@ -65,6 +66,7 @@ struct Opts {
     uint64_t cluster_seed = 0;                         // --cluster-seed S
     bool cluster_restarts_given = false, cluster_seed_given = false;
     std::string out_cluster_genotypes, out_cluster_matches;     // --out-cluster-genotypes FILE, --out-cluster-matches FILE
+    std::string out_cluster_calls;                              // --out-cluster-calls FILE
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
     uint32_t min_base_quality = 0;     // --min-base-quality (0: off)
@@ -103,6 +105,9 @@ void usage()
          "                              GT:GQ:PL per cluster), fitted together with the pool's ambient-RNA fraction\n"
          "      --out-cluster-matches FILE  With --out-clusters: match each cluster's genotypes against the VCF's samples (TSV, one\n"
          "                              line per cluster: best and second sample, their log-likelihood ratio, discordant calls)\n"
+         "      --out-cluster-calls FILE  With --out-clusters: each cell called against its cluster's genotypes and the pool's\n"
+         "                              ambient RNA, the clusters refit from their singlets until the calls settle (8 rounds at\n"
+         "                              most); the --out-donors columns, with the clusters as donors\n"
          "  -p, --padding INT           Padding on both sides of the variant [100]\n"
          "  -s, --scoring-method M      consensus | coverage | alt_frac [consensus]\n"
          "      --ref-matrix FILE       Reference matrix (coverage mode) [ref_matrix.mtx]\n"
@@ -208,6 +213,7 @@ bool parse(int argc, char** argv, Opts* o)
         else if (a == "--out-cluster-alleles") o->out_cluster_alleles = v();
         else if (a == "--out-cluster-genotypes") o->out_cluster_genotypes = v();
         else if (a == "--out-cluster-matches") o->out_cluster_matches = v();
+        else if (a == "--out-cluster-calls") o->out_cluster_calls = v();
         else if (a == "--clusters" || a == "--cluster-restarts" || a == "--cluster-seed") {
             const std::string t = v();
             char* end = nullptr;
@@ -304,6 +310,14 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --out-cluster-genotypes and --out-cluster-matches fit what the GPU run counts: they cannot be combined with --dump-staged\n");
         return false;
     }
+    if (o->out_clusters.empty() && !o->out_cluster_calls.empty()) {
+        fprintf(stderr, "error: --out-cluster-calls only applies with --out-clusters\n");
+        return false;
+    }
+    if (!o->out_cluster_calls.empty() && !o->dump_staged.empty()) {
+        fprintf(stderr, "error: --out-cluster-calls calls what the GPU run counts: it cannot be combined with --dump-staged\n");
+        return false;
+    }
     if (!o->out_clusters.empty() && !o->dump_staged.empty()) {
         fprintf(stderr, "error: --out-clusters clusters what the GPU run counts: it cannot be combined with --dump-staged\n");
         return false;
@@ -335,6 +349,7 @@ void check_inputs_exist(const Opts& o)
     if (!o.out_cluster_alleles.empty()) validate_output_path(o.out_cluster_alleles);
     if (!o.out_cluster_genotypes.empty()) validate_output_path(o.out_cluster_genotypes);
     if (!o.out_cluster_matches.empty()) validate_output_path(o.out_cluster_matches);
+    if (!o.out_cluster_calls.empty()) validate_output_path(o.out_cluster_calls);
     if (!exists(o.fasta + ".fai")) { LOG_ERR("File %s.fai does not exist", o.fasta.c_str()); exit(1); }
     const size_t dot = o.bam.find_last_of('.');
     const std::string ext = dot == std::string::npos ? "" : o.bam.substr(dot + 1);
@@ -683,6 +698,40 @@ int cluster_genotypes(const Opts& o, vtx_ctx* ctx, const vtx_result& res, const 
     LOG_INFO("Cluster genotypes: ambient RNA %.3f (estimated, %u fractions evaluated); rows fit: %llu; touched rows: %llu of %zu; genotypes called at GQ >= 20: %llu%s%s",
              cg.rho_permille / 1000.0, cg.n_evaluated, (unsigned long long)cg.rows_fit, (unsigned long long)cg.n_touched, recs.size(),
              (unsigned long long)called, matches ? "; assignments: " : "", assigned.c_str());
+    return rc;
+}
+
+// --out-cluster-calls: once, on lane 0, after the clustering, over the same entries (DESIGN.md §5j).  The error rate is §5f's
+// default and the loop stops after 8 rounds after round 0 at most.
+int cluster_calls(const Opts& o, vtx_ctx* ctx, const vtx_result& res, const std::vector<VcfRecord>& recs,
+                  const std::vector<std::string>& barcodes, const vtx_clusters& cl)
+{
+    constexpr uint32_t kRounds = 8;
+    const vtx_cluster_calls_params p{ cl.k, 0.01, kRounds };
+    vtx_cluster_calls cc{};
+    if (vtx_cluster_refine(ctx, res.n, res.row, res.col, res.ref_cnt, res.alt_cnt, recs.size(), uint32_t(barcodes.size()), cl.alt_w,
+                           cl.depth_w, cl.row_used, &p, &cc) != VTX_OK) {
+        printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx));
+        return 1;
+    }
+    int rc = 0;
+    validate_output_path(o.out_cluster_calls);
+    std::vector<std::string> names;
+    for (uint32_t j = 0; j < cc.k; ++j) names.push_back("C" + std::to_string(j));
+    const std::vector<int64_t> ll(cc.ll, cc.ll + size_t(cc.n_cols) * cc.n_hyp);
+    const std::vector<uint64_t> cnt(cc.counts, cc.counts + size_t(cc.n_cols) * 3);
+    uint64_t calls[3] = { 0, 0, 0 };
+    if (!write_donors(o.out_cluster_calls, barcodes, names, ll, cnt, calls)) { LOG_ERR("error writing cluster call file"); rc = 1; }
+    std::string rhos;
+    for (uint32_t r = 0; r < cc.n_rounds; ++r) {
+        char b[16];
+        snprintf(b, sizeof(b), "%s%.3f", r ? "," : "", cc.rounds[r].rho_permille / 1000.0);
+        rhos += b;
+    }
+    const vtx_cluster_calls_round& last = cc.rounds[cc.n_rounds - 1];
+    LOG_INFO("Cluster calls: ambient RNA per round %s; rounds: %u (%s); scored rows: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
+             rhos.c_str(), cc.n_rounds, cc.converged ? "converged" : "hit the cap", (unsigned long long)last.rows_scored, recs.size(),
+             (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
     return rc;
 }
 
@@ -1205,6 +1254,7 @@ int main(int argc, char** argv)
                      cl.k, o.cluster_restarts, (unsigned long long)o.cluster_seed, cl.best_restart, cl.restart_iters[cl.best_restart],
                      (unsigned long long)cl.rows_used, recs.size(), (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
             if (with_cluster_gt && cluster_genotypes(o, ctx, res, recs, gts, cl) != 0) rc = 1;
+            if (!o.out_cluster_calls.empty() && cluster_calls(o, ctx, res, recs, bcs.keys, cl) != 0) rc = 1;
         }
     }
     LOG_INFO("[%.3f s] outputs written", now_s());

@@ -11,6 +11,7 @@
 #include "vtx_clusters.cuh"
 #include "vtx_ambient.cuh"
 #include "vtx_cluster_gt.cuh"
+#include "vtx_cluster_refine.cuh"
 
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
@@ -171,7 +172,15 @@ struct vtx_ctx {
     std::vector<uint16_t> h_cg_m;
     std::vector<uint8_t> h_cg_gt;
     std::vector<uint32_t> h_cg_pl;
-    HostBuf h_stage;                                  // scalars read back between the staging phases
+    // vtx_cluster_refine: device work buffers (the entries, their indexes, sums, weights and cell outputs live in the cl_* buffers,
+    // the row sums in am_sums, the compacted fit in the cg_* buffers) and the host outputs of the last call
+    DBuf cr_rowflags, cr_code, cr_sflag, cr_scode, cr_tab, cr_label, cr_scal;
+    std::vector<int64_t> h_cr_ll;
+    std::vector<uint64_t> h_cr_cnt, h_cr_touched;
+    std::vector<uint32_t> h_cr_label, h_cr_pl;
+    std::vector<uint8_t> h_cr_gt;
+    std::vector<vtx_cluster_calls_round> h_cr_rounds;
+    HostBuf h_stage;                                 // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
 
@@ -1134,6 +1143,52 @@ int estimate_permille(std::vector<uint16_t>& ms, std::vector<int64_t>& obj, Eval
     if (rc) return rc;
     ms.insert(ms.end(), fine.begin(), fine.end());
     *chosen = best_of();
+    return VTX_OK;
+}
+
+// §5i's fit over touched rows already on the device: A / T [n_t][K], rowA / rowT [n_t], fit [n_fit] (touched indices of the used
+// rows).  given = -1 estimates m (ms / obj: every evaluated m in evaluation order), else fixes it.  At the chosen m, LL / GT / PL
+// [n_t][K] land in cg_ll / cg_gt / cg_pl.  J uses the first kMaxBatch entries of cg_acc, which the caller has sized.
+int cg_fit_device(vtx_ctx* ctx, const ambient::Fractions& fr, uint32_t K, int32_t given, uint32_t n_t, uint32_t n_fit, const uint32_t* d_fit,
+                  const unsigned long long* d_rowA, const unsigned long long* d_rowT, const int64_t* d_A, const int64_t* d_T,
+                  std::vector<uint16_t>& ms, std::vector<int64_t>& obj, uint32_t* chosen)
+{
+    using namespace cluster_gt;
+    cudaStream_t st = ctx->stream;
+    ENS(ctx->cg_ll, size_t(n_t) * K * 24 + 8);
+    ENS(ctx->cg_gt, size_t(n_t) * K + 8);
+    ENS(ctx->cg_pl, size_t(n_t) * K * 12 + 8);
+    unsigned long long* d_J = P<unsigned long long>(ctx->cg_acc);
+    // J(m) of every m in the list, one launch per batch of up to kMaxBatch
+    std::vector<unsigned long long> h_J(ambient::kMaxBatch);
+    auto evaluate = [&](const std::vector<uint16_t>& list) -> int {
+        for (size_t o = 0; o < list.size(); o += ambient::kMaxBatch) {
+            ambient::Batch bt{};
+            bt.n = uint32_t(std::min<size_t>(ambient::kMaxBatch, list.size() - o));
+            for (uint32_t b = 0; b < bt.n; ++b) bt.m[b] = list[o + b];
+            CK(cudaMemsetAsync(d_J, 0, size_t(ambient::kMaxBatch) * 8, st));
+            if (n_fit) {
+                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_fit * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
+                vtx_k_cg_fit<<<g, kCgThreads, 0, st>>>(bt, fr, K, n_fit, d_fit, d_rowA, d_rowT, d_A, d_T, d_J);
+                CK(cudaGetLastError());
+            }
+            CK(cudaMemcpyAsync(h_J.data(), d_J, size_t(bt.n) * 8, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            for (uint32_t b = 0; b < bt.n; ++b) obj.push_back(int64_t(h_J[b]));
+        }
+        return VTX_OK;
+    };
+    *chosen = uint32_t(given);
+    int rc = VTX_OK;
+    if (given < 0) rc = estimate_permille(ms, obj, evaluate, chosen);
+    else { ms.assign(1, uint16_t(*chosen)); rc = evaluate(ms); }
+    if (rc) return rc;
+    if (n_t) {
+        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_t) * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
+        vtx_k_cg_call<<<g, kCgThreads, 0, st>>>(*chosen, fr, K, n_t, d_rowA, d_rowT, d_A, d_T, P<int64_t>(ctx->cg_ll), P<uint8_t>(ctx->cg_gt),
+                                                 P<uint32_t>(ctx->cg_pl));
+        CK(cudaGetLastError());
+    }
     return VTX_OK;
 }
 
@@ -2104,9 +2159,6 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
     ENS(ctx->cg_AT, at.size() * 8 + 8);
     ENS(ctx->cg_rows, rows.size() * 8 + 8);
     ENS(ctx->cg_fit, size_t(n_fit) * 4 + 4);
-    ENS(ctx->cg_ll, size_t(n_t) * K * 24 + 8);
-    ENS(ctx->cg_gt, size_t(n_t) * K + 8);
-    ENS(ctx->cg_pl, size_t(n_t) * K * 12 + 8);
     ENS(ctx->cg_cmp, size_t(n_cmp) * 4 + 4);
     ENS(ctx->cg_dos, dos.size() + 8);
     ENS(ctx->cg_acc, (size_t(ambient::kMaxBatch) + 2 * size_t(K) * S + 2 * K) * 8);
@@ -2126,40 +2178,12 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
     unsigned long long* d_J = P<unsigned long long>(ctx->cg_acc);
     const ambient::Fractions fr = ambient::fractions(params->error_rate);
 
-    // J(m) of every m in the list, one launch per batch of up to kMaxBatch
+    // the fit and the calls at the chosen m, then the match
     std::vector<uint16_t> ms;
     std::vector<int64_t> obj;
-    std::vector<unsigned long long> h_J(ambient::kMaxBatch);
-    auto evaluate = [&](const std::vector<uint16_t>& list) -> int {
-        for (size_t o = 0; o < list.size(); o += ambient::kMaxBatch) {
-            ambient::Batch bt{};
-            bt.n = uint32_t(std::min<size_t>(ambient::kMaxBatch, list.size() - o));
-            for (uint32_t b = 0; b < bt.n; ++b) bt.m[b] = list[o + b];
-            CK(cudaMemsetAsync(d_J, 0, size_t(ambient::kMaxBatch) * 8, st));
-            if (n_fit) {
-                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_fit * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
-                vtx_k_cg_fit<<<g, kCgThreads, 0, st>>>(bt, fr, K, n_fit, P<uint32_t>(ctx->cg_fit), d_rowA, d_rowT, d_A, d_T, d_J);
-                CK(cudaGetLastError());
-            }
-            CK(cudaMemcpyAsync(h_J.data(), d_J, size_t(bt.n) * 8, cudaMemcpyDeviceToHost, st));
-            CK(cudaStreamSynchronize(st));
-            for (uint32_t b = 0; b < bt.n; ++b) obj.push_back(int64_t(h_J[b]));
-        }
-        return VTX_OK;
-    };
-    uint32_t chosen = uint32_t(given);
-    int rc = VTX_OK;
-    if (given < 0) rc = estimate_permille(ms, obj, evaluate, &chosen);
-    else { ms.assign(1, uint16_t(chosen)); rc = evaluate(ms); }
+    uint32_t chosen = 0;
+    const int rc = cg_fit_device(ctx, fr, K, given, n_t, n_fit, P<uint32_t>(ctx->cg_fit), d_rowA, d_rowT, d_A, d_T, ms, obj, &chosen);
     if (rc) return rc;
-
-    // the calls at the chosen m, then the match
-    if (n_t) {
-        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_t) * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
-        vtx_k_cg_call<<<g, kCgThreads, 0, st>>>(chosen, fr, K, n_t, d_rowA, d_rowT, d_A, d_T, P<int64_t>(ctx->cg_ll), P<uint8_t>(ctx->cg_gt),
-                                                 P<uint32_t>(ctx->cg_pl));
-        CK(cudaGetLastError());
-    }
     unsigned long long* d_M = d_J + ambient::kMaxBatch;
     const size_t n_acc = 2 * size_t(K) * S + 2 * K;                   // M, discordant [K][S], then rows, called [K]
     CK(cudaMemsetAsync(d_M, 0, n_acc * 8, st));
@@ -2200,6 +2224,264 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
     out->touched = ctx->h_cg_touched.data(); out->gt = ctx->h_cg_gt.data(); out->pl = ctx->h_cg_pl.data();
     out->match_ll = ctx->h_cg_M.data(); out->match_discordant = ctx->h_cg_acc.data() + size_t(K) * S;
     out->match_rows = ctx->h_cg_acc.data() + 2 * size_t(K) * S; out->match_called = out->match_rows + K;
+    return VTX_OK;
+}
+
+int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                       const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const int64_t* alt_w, const int64_t* depth_w,
+                       const uint8_t* row_used, const vtx_cluster_calls_params* params, vtx_cluster_calls* out)
+{
+    using namespace cluster_refine;
+    if (!ctx || !params || !out) return VTX_E_INVALID;
+    *out = vtx_cluster_calls{};
+    if (!ctx->finished || ctx->gather_pending)
+        return set_err(ctx, VTX_E_STATE, "vtx_cluster_refine: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const uint32_t K = params->k, max_rounds = params->max_rounds;
+    if (K < clusters::kMinK || K > clusters::kMaxK)
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: k = %u; 2 to 32 clusters are supported", K);
+    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: error rate %g outside [1e-6, 0.25]", params->error_rate);
+    if (max_rounds > kMaxRounds) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: max_rounds %u; 0 to 32 are supported", max_rounds);
+    if (n && (!row || !col || !ref_cnt || !alt_cnt)) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: an entry array is NULL");
+    if (n_rows && (!alt_w || !depth_w || !row_used)) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: a row array is NULL");
+    if (n > 0xFFFFFFFFull || n_rows > 0xFFFFFFFFull)
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: %llu entries over %llu rows; both must be below 2^32",
+                       (unsigned long long)n, (unsigned long long)n_rows);
+    const uint32_t H = donors::n_hyp(K);
+    // device memory, before any host table of n_rows entries: the entries (16 B) and their by-cell copy (12 B); per row the flags,
+    // scans, row sums and the round's sums, and at most every row touched and scored (the compacted fit, codes and tables); per
+    // cell the weights, labels, log-likelihoods and counts.  Every buffer is allocated with 1/8 to spare (ensure).
+    {
+        const double need = (double(n) * 28 + double(n_rows) * (70.0 * K + 150) + double(n_cols) * (4.0 * K + 8.0 * H + 40) + 4096) * 1.125;
+        CK(cudaSetDevice(ctx->device));
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        size_t held = 0;
+        for (DBuf* b : { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_row_start, &ctx->cl_cell_count,
+                         &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_w, &ctx->cl_A, &ctx->cl_T, &ctx->cl_ll,
+                         &ctx->cl_cnt, &ctx->am_sums, &ctx->cg_AT, &ctx->cg_rows, &ctx->cg_fit, &ctx->cg_ll, &ctx->cg_gt, &ctx->cg_pl,
+                         &ctx->cg_acc, &ctx->cr_rowflags, &ctx->cr_code, &ctx->cr_sflag, &ctx->cr_scode, &ctx->cr_tab, &ctx->cr_label,
+                         &ctx->cr_scal })
+            held += b->cap;
+        if (need > double(free_b) + double(held))
+            return set_err(ctx, VTX_E_NOMEM, "vtx_cluster_refine needs %.0f MB of device memory, %.0f MB are free", need * 1e-6,
+                           (double(free_b) + double(held)) * 1e-6);
+    }
+    // validate once: §5i's bounds on the sums, then the entries, whose total bounds every later round's hard sums
+    uint64_t total = 0;
+    for (uint64_t v = 0; v < n_rows; ++v)
+        for (uint32_t k = 0; k < K; ++k) {
+            const int64_t a = alt_w[v * K + k], t = depth_w[v * K + k];
+            if (a < 0 || a > t || t > cluster_gt::kMaxDepthW)
+                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: row %llu, cluster %u: alt_w %lld, depth_w %lld (0 <= alt_w <= depth_w <= 2^51)",
+                               (unsigned long long)v, k, (long long)a, (long long)t);
+            total += uint64_t(t);
+            if (total > cluster_gt::kMaxTotalDepthW)
+                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: depth_w sums to more than 2^51 over the rows; the fit's int64 sums would not be exact");
+        }
+    std::vector<uint32_t> row_start(size_t(n_rows) + 1, 0);
+    uint64_t molecules = 0;
+    int rc = validate_entries(ctx, "vtx_cluster_refine", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxTotalMolecules,
+                              "its hard sums would not be exact", [&](uint32_t v, uint64_t i0, uint64_t i1, uint64_t m) {
+        row_start[size_t(v) + 1] = uint32_t(i1 - i0);
+        molecules += m;
+    });
+    if (rc) return rc;
+    if (molecules > kMaxTotalMolecules)
+        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: the entries hold more than 2^35 molecules; the fit's int64 sums would not be exact");
+    for (uint64_t v = 0; v < n_rows; ++v) row_start[v + 1] += row_start[v];
+
+    cudaStream_t st = ctx->stream;
+    const size_t nb = size_t(n) * 4 + 4;
+    ENS(ctx->cl_row, nb); ENS(ctx->cl_col, nb); ENS(ctx->cl_r, nb); ENS(ctx->cl_a, nb);
+    ENS(ctx->cl_c_row, nb); ENS(ctx->cl_c_r, nb); ENS(ctx->cl_c_a, nb);
+    ENS(ctx->cl_used, size_t(n_rows) + 1);
+    ENS(ctx->cl_row_start, row_start.size() * 4);
+    ENS(ctx->cl_cell_count, (size_t(n_cols) + 1) * 4);
+    ENS(ctx->cl_cell_start, (size_t(n_cols) + 1) * 4);
+    ENS(ctx->cl_w, size_t(n_cols) * K * 4 + 4);
+    ENS(ctx->cl_A, size_t(n_rows) * K * 8 + 8); ENS(ctx->cl_T, size_t(n_rows) * K * 8 + 8);
+    ENS(ctx->cl_ll, size_t(n_cols) * H * 8 + 8); ENS(ctx->cl_cnt, size_t(n_cols) * 24 + 8);
+    ENS(ctx->am_sums, size_t(n_rows) * 16 + 16);
+    ENS(ctx->cg_acc, size_t(ambient::kMaxBatch) * 8);
+    const size_t rf = size_t(n_rows) + 1;                   // tflag, tpos, fflag, fpos, sidx: n_rows + 1 each
+    ENS(ctx->cr_rowflags, rf * 5 * 4);
+    ENS(ctx->cr_label, size_t(n_cols) * 8 + 8);
+    ENS(ctx->cr_scal, 4 * 8);
+    if (n) {
+        CK(cudaMemcpyAsync(ctx->cl_row.p, row, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_r.p, ref_cnt, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_a.p, alt_cnt, n * 4, cudaMemcpyHostToDevice, st));
+    }
+    CK(cudaMemcpyAsync(ctx->cl_row_start.p, row_start.data(), row_start.size() * 4, cudaMemcpyHostToDevice, st));
+    if (n_rows) {
+        CK(cudaMemcpyAsync(ctx->cl_A.p, alt_w, size_t(n_rows) * K * 8, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_T.p, depth_w, size_t(n_rows) * K * 8, cudaMemcpyHostToDevice, st));
+    }
+    unsigned long long* d_rowA = P<unsigned long long>(ctx->am_sums);
+    unsigned long long* d_rowT = d_rowA + n_rows;
+    CK(cudaMemsetAsync(ctx->am_sums.p, 0, size_t(n_rows) * 16, st));
+
+    // A_v, T_v and the by-cell index of every entry with r + a > 0 (§5g's kernels with every row kept); then `used` becomes row_used
+    const uint32_t nn = uint32_t(n);
+    const unsigned egrid = std::max(1u, std::min(blocks_for(n, kCrThreads), unsigned(ctx->n_sm) * 16));
+    if (n) {
+        ambient::vtx_k_am_rowsum<<<egrid, kCrThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a), d_rowA, d_rowT);
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemsetAsync(ctx->cl_used.p, 1, size_t(n_rows) + 1, st));
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    clusters::vtx_k_cl_count<<<egrid, kCrThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                           P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_count));
+    CK(cudaGetLastError());
+    rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->cl_cell_count), n_cols, P<uint32_t>(ctx->cl_cell_start), nullptr);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    clusters::vtx_k_cl_scatter<<<egrid, kCrThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                             P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_start),
+                                                             P<uint32_t>(ctx->cl_cell_count), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r),
+                                                             P<uint32_t>(ctx->cl_c_a));
+    CK(cudaGetLastError());
+    if (n_rows) CK(cudaMemcpyAsync(ctx->cl_used.p, row_used, n_rows, cudaMemcpyHostToDevice, st));
+    const clusters::CellEntries ce{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
+    uint32_t* d_tflag = P<uint32_t>(ctx->cr_rowflags);
+    uint32_t* d_tpos = d_tflag + rf;
+    uint32_t* d_fflag = d_tpos + rf;
+    uint32_t* d_fpos = d_fflag + rf;
+    uint32_t* d_sidx = d_fpos + rf;
+    uint32_t* d_label = P<uint32_t>(ctx->cr_label);
+    uint32_t* d_prev = d_label + n_cols;
+    unsigned long long* d_scal = P<unsigned long long>(ctx->cr_scal);       // calls [3], changed
+    CK(cudaMemsetAsync(d_prev, 0xFF, size_t(n_cols) * 4, st));              // round 0 compares with VTX_NO_LABEL
+
+    const ambient::Fractions fr = ambient::fractions(params->error_rate);
+    const unsigned rgrid = std::max(1u, std::min(blocks_for(n_rows, kCrThreads), unsigned(ctx->n_sm) * 16));
+    clusters::Perm ident{};
+    for (uint32_t k = 0; k < K; ++k) ident.k[k] = uint8_t(k);
+    ctx->h_cr_rounds.clear();
+    bool converged = false;
+    uint32_t n_t = 0;
+    for (uint32_t r = 0;; ++r) {
+        if (r > 0 && n_rows) {       // the previous round's labels' hard sums
+            const unsigned g = std::max(1u, std::min(blocks_for(n_rows * 32, clusters::kClThreads), unsigned(ctx->n_sm) * 16));
+            clusters::vtx_k_cl_final<<<g, clusters::kClThreads, 0, st>>>(ident, n_rows, P<uint32_t>(ctx->cl_row_start), P<uint32_t>(ctx->cl_col),
+                                                                         P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a), P<uint32_t>(ctx->cl_w), K,
+                                                                         P<int64_t>(ctx->cl_A), P<int64_t>(ctx->cl_T));
+            CK(cudaGetLastError());
+        }
+        // the touched and fitted rows, compacted on the device
+        uint32_t counts[2] = { 0, 0 };
+        if (n_rows) {
+            vtx_k_cr_touch<<<rgrid, kCrThreads, 0, st>>>(n_rows, K, P<int64_t>(ctx->cl_T), P<uint8_t>(ctx->cl_used), d_tflag, d_fflag);
+            CK(cudaGetLastError());
+            rc = scan_u32(ctx, st, ctx->scan_sums, d_tflag, n_rows, d_tpos, nullptr);
+            if (rc) return rc;
+            rc = scan_u32(ctx, st, ctx->scan_sums, d_fflag, n_rows, d_fpos, nullptr);
+            if (rc) return rc;
+            CK(cudaMemcpyAsync(&counts[0], d_tpos + n_rows, 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(&counts[1], d_fpos + n_rows, 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+        }
+        n_t = counts[0];
+        const uint32_t n_fit = counts[1];
+        ENS(ctx->cg_AT, size_t(n_t) * K * 16 + 8);
+        ENS(ctx->cg_rows, size_t(n_t) * 16 + 8);
+        ENS(ctx->cg_fit, size_t(n_fit) * 4 + 4);
+        ENS(ctx->cr_sflag, (size_t(n_t) * 3 + 1) * 4);        // sflag, spos (n_t + 1), trow
+        ENS(ctx->cr_code, size_t(n_t) * K + 8);
+        int64_t* d_cA = P<int64_t>(ctx->cg_AT);
+        int64_t* d_cT = d_cA + size_t(n_t) * K;
+        unsigned long long* d_crow = P<unsigned long long>(ctx->cg_rows);
+        uint32_t* d_sflag = P<uint32_t>(ctx->cr_sflag);
+        uint32_t* d_spos = d_sflag + n_t;
+        uint32_t* d_trow = d_spos + n_t + 1;
+        if (n_t) {
+            vtx_k_cr_gather<<<rgrid, kCrThreads, 0, st>>>(n_rows, K, n_t, P<int64_t>(ctx->cl_A), P<int64_t>(ctx->cl_T), d_rowA, d_rowT, d_tflag,
+                                                          d_tpos, d_fflag, d_fpos, d_cA, d_cT, d_crow, d_trow, P<uint32_t>(ctx->cg_fit));
+            CK(cudaGetLastError());
+        }
+        // §5i's fit and calls, then the codes and the scored rows' tables
+        std::vector<uint16_t> ms;
+        std::vector<int64_t> obj;
+        uint32_t m = 0;
+        rc = cg_fit_device(ctx, fr, K, -1, n_t, n_fit, P<uint32_t>(ctx->cg_fit), d_crow, d_crow + n_t, d_cA, d_cT, ms, obj, &m);
+        if (rc) return rc;
+        uint32_t n_s = 0;
+        if (n_t) {
+            const unsigned g = std::max(1u, std::min(blocks_for(n_t, kCrThreads), unsigned(ctx->n_sm) * 16));
+            vtx_k_cr_codes<<<g, kCrThreads, 0, st>>>(n_t, K, P<uint8_t>(ctx->cg_gt), P<uint32_t>(ctx->cg_pl), P<uint8_t>(ctx->cr_code), d_sflag);
+            CK(cudaGetLastError());
+            rc = scan_u32(ctx, st, ctx->scan_sums, d_sflag, n_t, d_spos, nullptr);
+            if (rc) return rc;
+            CK(cudaMemcpyAsync(&n_s, d_spos + n_t, 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+        }
+        ENS(ctx->cr_scode, size_t(n_s) * K + 8);
+        ENS(ctx->cr_tab, size_t(n_s) * kEntries * 8 + 8);
+        if (n_rows) CK(cudaMemsetAsync(d_sidx, 0xFF, size_t(n_rows) * 4, st));
+        if (n_s) {
+            const unsigned g = std::max(1u, std::min(blocks_for(n_t, kCrThreads), unsigned(ctx->n_sm) * 16));
+            vtx_k_cr_tables<<<g, kCrThreads, 0, st>>>(m, fr, n_t, K, d_trow, d_crow, P<uint8_t>(ctx->cr_code), d_sflag, d_spos, d_sidx,
+                                                      P<uint8_t>(ctx->cr_scode), P<int32_t>(ctx->cr_tab));
+            CK(cudaGetLastError());
+        }
+        // the cells: scores, calls and labels; the next round's weights and the changed labels
+        CK(cudaMemsetAsync(d_scal, 0, 4 * 8, st));
+        if (n_cols) {
+            const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_cols) * 32, kCrThreads), unsigned(ctx->n_sm) * 8));
+            const uint32_t* sx = d_sidx;
+            const uint8_t* sc = P<uint8_t>(ctx->cr_scode);
+            const int32_t* tb = P<int32_t>(ctx->cr_tab);
+            int64_t* ll = P<int64_t>(ctx->cl_ll);
+            uint64_t* cnt = P<uint64_t>(ctx->cl_cnt);
+            if (H <= 32) vtx_k_cr_score<1><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
+            else if (H <= 64) vtx_k_cr_score<2><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
+            else if (H <= 160) vtx_k_cr_score<5><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
+            else if (H <= 288) vtx_k_cr_score<9><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
+            else vtx_k_cr_score<17><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
+            CK(cudaGetLastError());
+            const unsigned wg = std::max(1u, std::min(blocks_for(n_cols, kCrThreads), unsigned(ctx->n_sm) * 16));
+            vtx_k_cr_weights<<<wg, kCrThreads, 0, st>>>(n_cols, K, d_label, d_prev, P<uint32_t>(ctx->cl_w), d_scal + 3);
+            CK(cudaGetLastError());
+        }
+        unsigned long long h_scal[4];
+        CK(cudaMemcpyAsync(h_scal, d_scal, sizeof(h_scal), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        vtx_cluster_calls_round rr{};
+        rr.rho_permille = m; rr.rows_fit = n_fit; rr.n_touched = n_t; rr.rows_scored = n_s;
+        for (int i = 0; i < 3; ++i) rr.calls[i] = h_scal[i];
+        rr.changed = h_scal[3];
+        ctx->h_cr_rounds.push_back(rr);
+        if (r > 0 && rr.changed == 0) { converged = true; break; }
+        if (r == max_rounds) break;
+    }
+
+    // the last round's cells and fit
+    ctx->h_cr_ll.resize(size_t(n_cols) * H);
+    ctx->h_cr_cnt.resize(size_t(n_cols) * 3);
+    ctx->h_cr_label.resize(n_cols);
+    std::vector<uint32_t> trow(n_t);
+    ctx->h_cr_gt.resize(size_t(n_t) * K);
+    ctx->h_cr_pl.resize(size_t(n_t) * K * 3);
+    if (n_cols) {
+        CK(cudaMemcpyAsync(ctx->h_cr_ll.data(), ctx->cl_ll.p, ctx->h_cr_ll.size() * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_cr_cnt.data(), ctx->cl_cnt.p, ctx->h_cr_cnt.size() * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_cr_label.data(), d_label, size_t(n_cols) * 4, cudaMemcpyDeviceToHost, st));
+    }
+    if (n_t) {
+        CK(cudaMemcpyAsync(trow.data(), P<uint32_t>(ctx->cr_sflag) + 2 * size_t(n_t) + 1, size_t(n_t) * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_cr_gt.data(), ctx->cg_gt.p, ctx->h_cr_gt.size(), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_cr_pl.data(), ctx->cg_pl.p, ctx->h_cr_pl.size() * 4, cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    ctx->h_cr_touched.assign(trow.begin(), trow.end());
+
+    out->k = K; out->n_cols = n_cols; out->n_hyp = H; out->n_rounds = uint32_t(ctx->h_cr_rounds.size()); out->converged = converged;
+    out->n_rows = n_rows; out->n_touched = n_t;
+    out->ll = ctx->h_cr_ll.data(); out->counts = ctx->h_cr_cnt.data(); out->label = ctx->h_cr_label.data();
+    out->rounds = ctx->h_cr_rounds.data();
+    out->touched = ctx->h_cr_touched.data(); out->gt = ctx->h_cr_gt.data(); out->pl = ctx->h_cr_pl.data();
     return VTX_OK;
 }
 

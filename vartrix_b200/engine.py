@@ -722,6 +722,47 @@ class Engine:
                     match_ll=arr(out.match_ll, k * s, np.int64, (k, s)), match_discordant=arr(out.match_discordant, k * s, np.uint64, (k, s)),
                     match_rows=arr(out.match_rows, k, np.uint64, (k,)), match_called=arr(out.match_called, k, np.uint64, (k,)))
 
+    def cluster_refine(self, row, col, ref, alt, n_rows: int, n_cols: int, clusters: dict, error_rate: float = 0.01,
+                       max_rounds: int = 8) -> dict:
+        """The cells called against their clusters' fitted genotypes and ambient RNA, with the clusters refit from their singlets
+        (vtx_cluster_refine, include/vartrix_b200.h; DESIGN.md §5j): count entries as cluster_cells takes them, and the dict
+        cluster_cells returned for them.  -> dict of NumPy copies: ll int64[n_cols, H] (x 2^24) and counts uint64[n_cols, 3] of the
+        last round, label uint32[n_cols] (NO_LABEL unless singlet), rho_permille / rows_fit / n_touched / rows_scored / changed
+        int64[rounds] and calls int64[rounds, 3] per round, the last round's touched uint64[n_touched], gt uint8[n_touched, k] and
+        pl uint32[n_touched, k, 3], and the scalars k, n_hyp, n_rounds, converged."""
+        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
+        n = len(arrs[0])
+        if any(len(x) != n for x in arrs):
+            raise ValueError("row, col, ref and alt must have the same length")
+        A = np.ascontiguousarray(clusters["alt_w"], dtype=np.int64)
+        T = np.ascontiguousarray(clusters["depth_w"], dtype=np.int64)
+        used = np.ascontiguousarray(clusters["row_used"], dtype=np.uint8)
+        if A.ndim != 2 or A.shape != T.shape or A.shape[0] != int(n_rows) or used.shape != (int(n_rows),):
+            raise ValueError("clusters must hold alt_w / depth_w [n_rows, k] and row_used [n_rows]")
+        k = A.shape[1]
+        out = _capi.ClusterCalls()
+        p = _capi.ClusterCallsParams(k, float(error_rate), int(max_rounds))
+        ptr = [x.ctypes.data if n else None for x in arrs] + [x.ctypes.data if int(n_rows) else None for x in (A, T, used)]
+        self._ck(self._L.vtx_cluster_refine(self._h, n, *ptr[:4], int(n_rows), int(n_cols), *ptr[4:], C.byref(p), C.byref(out)),
+                 "vtx_cluster_refine")
+
+        def arr(ptr, count, dtype, shape):
+            if count == 0:
+                return np.zeros(shape, dtype)
+            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
+        nc, nh, nt, nr = int(out.n_cols), int(out.n_hyp), int(out.n_touched), int(out.n_rounds)
+        rounds = [out.rounds[i] for i in range(nr)]
+        return dict(k=k, n_hyp=nh, n_rounds=nr, converged=bool(out.converged),
+                    ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
+                    label=arr(out.label, nc, np.uint32, (nc,)),
+                    rho_permille=np.array([x.rho_permille for x in rounds], np.int64),
+                    rows_fit=np.array([x.rows_fit for x in rounds], np.int64), n_touched=np.array([x.n_touched for x in rounds], np.int64),
+                    rows_scored=np.array([x.rows_scored for x in rounds], np.int64),
+                    calls=np.array([list(x.calls) for x in rounds], np.int64).reshape(nr, 3),
+                    changed=np.array([x.changed for x in rounds], np.int64),
+                    touched=arr(out.touched, nt, np.uint64, (nt,)), gt=arr(out.gt, nt * k, np.uint8, (nt, k)),
+                    pl=arr(out.pl, nt * k * 3, np.uint32, (nt, k, 3)))
+
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()
 
