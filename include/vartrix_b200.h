@@ -414,6 +414,29 @@ int         vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, con
                               const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params,
                               vtx_clusters* out);
 
+/* ---- clustering of a pool where some donors are genotyped (the CLI's --known-donors; DESIGN.md §5k) --------------------------
+ * vtx_cluster_cells' model over the same entries, with the first n_pinned = J clusters (1 <= J <= k - 1) pinned to samples of
+ * known genotype: dosage [row * J + j] is 0, 1, 2 or VTX_GT_MISSING for every row < n_rows.  Where sample j has a dosage g at
+ * row v, cluster j is not fitted: it expects vtx_donors_ambient's contaminated fraction theta_jv = (1 - rho) q_2g + rho f_v
+ * (q_0, q_2, q_4 = error_rate, 0.5, 1 - error_rate; f_v the pool's ALT fraction over every entry at row v; rho = m / 1000 with
+ * m = rho_permille, given), with vtx_donors_ambient's int32 logs, for the whole EM; the scoring mixes that theta into the
+ * doublets as it mixes every other cluster's.  Where sample j has no dosage, cluster j is an ordinary cluster of that row.
+ * Clusters 0 .. J - 1 keep their indices (the samples' order); clusters J .. k - 1 are free and ordered among themselves by
+ * sum_c W_ck, descending (ties: EM index).  alt_w / depth_w hold the winner's final A, T of every cluster, pinned ones included.
+ *
+ * out is filled as vtx_cluster_cells fills it, library-owned host memory valid until the next vtx_cluster_cells,
+ * vtx_cluster_cells_pinned or vtx_destroy.  Device memory: vtx_cluster_cells' plus J + 16 bytes per row.  VTX_E_STATE while
+ * submits are unfinished; VTX_E_INVALID for vtx_cluster_cells' refusals, n_pinned outside 1 .. k - 1, a NULL dosage, a dosage
+ * other than 0, 1, 2 or VTX_GT_MISSING, error_rate outside [1e-6, 0.25] or rho_permille outside 0 .. 500 (a row's T_v + 2
+ * stays below 2^53: vtx_cluster_cells' bound on a row's molecules is far lower); VTX_E_NOMEM when the device cannot hold it. */
+typedef struct vtx_cluster_pinned_params {
+    uint32_t k, restarts; uint64_t seed;
+    uint32_t n_pinned; double error_rate; int32_t rho_permille;
+} vtx_cluster_pinned_params;
+int         vtx_cluster_cells_pinned(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                                     const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const uint8_t* dosage,
+                                     const vtx_cluster_pinned_params* params, vtx_clusters* out);
+
 /* ---- donor assignment against ambient RNA (the CLI's --ambient-rna; DESIGN.md §5h) -----------------------------------------
  * vtx_set_donors' model over host count entries (row, col, ref_cnt, alt_cnt) as vtx_cluster_cells takes them, with the pool's
  * ALT fraction mixed into every hypothesis: at row v, q_vs = (1 - rho) q_s + rho f_v and 1 - q_vs = (1 - rho)(1 - q_s) +

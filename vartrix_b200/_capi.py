@@ -32,7 +32,7 @@ SYMBOLS = [
     "vtx_comm_unique_id", "vtx_comm_init", "vtx_gather", "vtx_gather_start", "vtx_gather_wait",
     "vtx_submit2", "vtx_submit2_device", "vtx_pack_cb", "vtx_bgzf_inflate", "vtx_submit_bam", "vtx_bam_metrics_get",
     "vtx_set_min_base_quality", "vtx_bam_low_base_quality", "vtx_set_locus_stats", "vtx_locus_stats_get",
-    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells", "vtx_donors_ambient", "vtx_cluster_genotypes", "vtx_cluster_refine",
+    "vtx_set_donors", "vtx_donor_ll_get", "vtx_cluster_cells", "vtx_cluster_cells_pinned", "vtx_donors_ambient", "vtx_cluster_genotypes", "vtx_cluster_refine",
 ]
 NO_CB_KEY = 0xFFFFFFFFFFFFFFFF
 NO_LABEL = 0xFFFFFFFF     # VTX_NO_LABEL: a cell vtx_cluster_refine did not call singlet
@@ -117,6 +117,11 @@ class Clusters(C.Structure):       # vtx_clusters
                 ("n_rows", C.c_uint64), ("rows_used", C.c_uint64), ("ll", C.POINTER(C.c_int64)), ("counts", C.POINTER(C.c_uint64)),
                 ("row_used", C.POINTER(C.c_uint8)), ("alt_w", C.POINTER(C.c_int64)), ("depth_w", C.POINTER(C.c_int64)),
                 ("restart_score", C.POINTER(C.c_int64)), ("restart_iters", C.POINTER(C.c_uint32))]
+
+
+class ClusterPinnedParams(C.Structure):    # vtx_cluster_pinned_params
+    _fields_ = [("k", C.c_uint32), ("restarts", C.c_uint32), ("seed", C.c_uint64), ("n_pinned", C.c_uint32),
+                ("error_rate", C.c_double), ("rho_permille", C.c_int32)]
 
 
 class AmbientParams(C.Structure):  # vtx_ambient_params
@@ -245,6 +250,9 @@ def load():
     L.vtx_cluster_cells.restype = C.c_int
     L.vtx_cluster_cells.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                                     C.POINTER(ClusterParams), C.POINTER(Clusters)]
+    L.vtx_cluster_cells_pinned.restype = C.c_int
+    L.vtx_cluster_cells_pinned.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                           C.c_void_p, C.POINTER(ClusterPinnedParams), C.POINTER(Clusters)]
     L.vtx_donors_ambient.restype = C.c_int
     L.vtx_donors_ambient.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                                      C.c_void_p, C.POINTER(AmbientParams), C.POINTER(Ambient)]

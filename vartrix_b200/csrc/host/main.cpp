@@ -67,6 +67,8 @@ struct Opts {
     bool cluster_restarts_given = false, cluster_seed_given = false;
     std::string out_cluster_genotypes, out_cluster_matches;     // --out-cluster-genotypes FILE, --out-cluster-matches FILE
     std::string out_cluster_calls;                              // --out-cluster-calls FILE
+    std::string known_donors;                                   // --known-donors NAME,NAME,...
+    std::vector<std::string> known;                             // ... split, in list order
     long padding = 100, threads = 1, mapq = 0, device = 0, shard_loci = 0;      // 0: chosen from the number of loci and threads
     long shard_bytes = 0;       // compressed BAM bytes a shard may span (0: no limit; 192 MB under --gpu-stage)
     uint32_t min_base_quality = 0;     // --min-base-quality (0: off)
@@ -91,9 +93,9 @@ void usage()
          "                              doublet log-likelihoods from the cell's REF / ALT counts, the best pair and the call\n"
          "      --donors LIST           The VCF samples that are the pool's donors, e.g. S1,S4,S2 (2 to 32) [every sample]\n"
          "      --donor-error-rate E    Per-molecule error rate of the donor model, 1e-6 .. 0.25 [0.01]\n"
-         "      --ambient-rna MODE      With --out-donors: model ambient RNA, molecules from the whole pool mixed into every cell.\n"
-         "                              MODE is 'estimate' (the fraction that fits the cells best) or a fraction 0 .. 0.5 with at\n"
-         "                              most three decimals\n"
+         "      --ambient-rna MODE      With --out-donors or --known-donors: model ambient RNA, molecules from the whole pool mixed\n"
+         "                              into every cell.  MODE is 'estimate' (the fraction that fits the cells best; --out-donors\n"
+         "                              only) or a fraction 0 .. 0.5 with at most three decimals\n"
          "      --out-ambient FILE      With --ambient-rna: the fit of every fraction evaluated (TSV: rho, objective, calls)\n"
          "      --out-clusters FILE     Cluster the cells into --clusters donors without genotypes (TSV, one line per barcode, the\n"
          "                              --out-donors columns with clusters C0, C1, ... for donors): allele-fraction EM, doublet calls\n"
@@ -108,6 +110,11 @@ void usage()
          "      --out-cluster-calls FILE  With --out-clusters: each cell called against its cluster's genotypes and the pool's\n"
          "                              ambient RNA, the clusters refit from their singlets until the calls settle (8 rounds at\n"
          "                              most); the --out-donors columns, with the clusters as donors\n"
+         "      --known-donors LIST     With --out-clusters: the VCF samples among the pool's donors, e.g. S1,S4 (1 to K - 1): their\n"
+         "                              clusters keep their VCF genotypes, come first and carry their names; the others are\n"
+         "                              fitted freely as C0, C1, ...  The model needs the ambient fraction: give it with\n"
+         "                              --ambient-rna (a fraction; 0 without it).  An unpinned run's --out-cluster-genotypes\n"
+         "                              reports an estimate of it, which reads high when the clusters mix donors\n"
          "  -p, --padding INT           Padding on both sides of the variant [100]\n"
          "  -s, --scoring-method M      consensus | coverage | alt_frac [consensus]\n"
          "      --ref-matrix FILE       Reference matrix (coverage mode) [ref_matrix.mtx]\n"
@@ -171,6 +178,51 @@ bool parse_ambient(const std::string& s, int32_t* permille)
     return true;
 }
 
+// --known-donors: the checks that need no VCF (its sample columns are checked once it is read)
+bool parse_known(Opts* o)
+{
+    if (o->out_clusters.empty()) { fprintf(stderr, "error: --known-donors only applies with --out-clusters\n"); return false; }
+    if (!o->dump_staged.empty()) {
+        fprintf(stderr, "error: --known-donors clusters what the GPU run counts: it cannot be combined with --dump-staged\n");
+        return false;
+    }
+    if (!o->out_cluster_genotypes.empty() || !o->out_cluster_matches.empty() || !o->out_cluster_calls.empty()) {
+        fprintf(stderr, "error: --known-donors cannot be combined with --out-cluster-genotypes, --out-cluster-matches or --out-cluster-calls\n");
+        return false;
+    }
+    if (!o->out_ambient.empty() && o->out_donors.empty()) {
+        fprintf(stderr, "error: --out-ambient only applies with --out-donors and --ambient-rna, not with --known-donors alone\n");
+        return false;
+    }
+    if (o->ambient_permille < 0 && !o->ambient_rna.empty()) {
+        fprintf(stderr, "error: --known-donors needs the ambient fraction given: --ambient-rna estimate does not apply with it\n");
+        return false;
+    }
+    for (size_t p = 0; p <= o->known_donors.size();) {
+        size_t q = o->known_donors.find(',', p);
+        if (q == std::string::npos) q = o->known_donors.size();
+        const std::string name = o->known_donors.substr(p, q - p);
+        if (name.empty()) { fprintf(stderr, "error: --known-donors: an empty sample name\n"); return false; }
+        if (std::find(o->known.begin(), o->known.end(), name) != o->known.end()) {
+            fprintf(stderr, "error: --known-donors: '%s' is listed twice\n", name.c_str());
+            return false;
+        }
+        o->known.push_back(name);
+        p = q + 1;
+    }
+    const size_t J = o->known.size();
+    if (J >= o->clusters) {
+        fprintf(stderr, "error: --known-donors lists %zu samples; with --clusters %u it takes 1 to %u\n", J, o->clusters, o->clusters - 1);
+        return false;
+    }
+    for (size_t j = 0; j < o->clusters - J; ++j)
+        if (std::find(o->known.begin(), o->known.end(), "C" + std::to_string(j)) != o->known.end()) {
+            fprintf(stderr, "error: --known-donors: 'C%zu' is also the name of a free cluster; rename the sample\n", j);
+            return false;
+        }
+    return true;
+}
+
 bool parse(int argc, char** argv, Opts* o)
 {
     auto need = [&](int& i) -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: %s needs a value\n", argv[i]); exit(1); } return argv[++i]; };
@@ -214,6 +266,10 @@ bool parse(int argc, char** argv, Opts* o)
         else if (a == "--out-cluster-genotypes") o->out_cluster_genotypes = v();
         else if (a == "--out-cluster-matches") o->out_cluster_matches = v();
         else if (a == "--out-cluster-calls") o->out_cluster_calls = v();
+        else if (a == "--known-donors") {
+            o->known_donors = v();
+            if (o->known_donors.empty()) { fprintf(stderr, "error: --known-donors needs at least one sample name\n"); return false; }
+        }
         else if (a == "--clusters" || a == "--cluster-restarts" || a == "--cluster-seed") {
             const std::string t = v();
             char* end = nullptr;
@@ -286,8 +342,8 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --donors and --donor-error-rate only apply with --out-donors\n");
         return false;
     }
-    if (!o->ambient_rna.empty() && o->out_donors.empty()) {
-        fprintf(stderr, "error: --ambient-rna only applies with --out-donors\n");
+    if (!o->ambient_rna.empty() && o->out_donors.empty() && o->known_donors.empty()) {
+        fprintf(stderr, "error: --ambient-rna only applies with --out-donors or --known-donors\n");
         return false;
     }
     if (!o->out_ambient.empty() && o->ambient_rna.empty()) {
@@ -318,6 +374,7 @@ bool parse(int argc, char** argv, Opts* o)
         fprintf(stderr, "error: --out-cluster-calls calls what the GPU run counts: it cannot be combined with --dump-staged\n");
         return false;
     }
+    if (!o->known_donors.empty() && !parse_known(o)) return false;
     if (!o->out_clusters.empty() && !o->dump_staged.empty()) {
         fprintf(stderr, "error: --out-clusters clusters what the GPU run counts: it cannot be combined with --dump-staged\n");
         return false;
@@ -536,6 +593,23 @@ bool select_donors(const std::string& list, const VcfGenotypes& g, const std::ve
     return true;
 }
 
+// --known-donors: the listed samples, in list order, and their dosage table (one row per VCF record = matrix row)
+bool select_known(const std::vector<std::string>& list, const VcfGenotypes& g, const std::vector<VcfRecord>& recs, DonorTable* t, std::string* err)
+{
+    std::vector<size_t> idx;
+    for (const std::string& name : list) {
+        const auto it = std::find(g.samples.begin(), g.samples.end(), name);
+        if (it == g.samples.end()) { *err = "--known-donors: '" + name + "' is not a sample column of the VCF"; return false; }
+        idx.push_back(size_t(it - g.samples.begin()));
+    }
+    const size_t ns = g.samples.size(), nd = idx.size();
+    t->names = list;
+    t->dosage.resize(recs.size() * nd);
+    for (size_t r = 0; r < recs.size(); ++r)
+        for (size_t d = 0; d < nd; ++d) t->dosage[r * nd + d] = g.dosage[r * ns + idx[d]];
+    return true;
+}
+
 // The donor file: one line per barcode in column order.  ll [col][H] and cnt [col][3] are the engine's sums over every lane.
 // The calls use the fixed threshold T = 5 nats, compared in the integer scale.
 bool write_donors(const std::string& path, const std::vector<std::string>& barcodes, const std::vector<std::string>& names,
@@ -586,12 +660,13 @@ bool write_ambient(const std::string& path, const vtx_ambient& am)
 }
 
 // --out-cluster-alleles: one line per VCF record in row order, the cluster's REF and ALT molecules (x 2^16 sums scaled back)
-bool write_cluster_alleles(const std::string& path, const std::vector<VcfRecord>& recs, const vtx_clusters& cl)
+bool write_cluster_alleles(const std::string& path, const std::vector<VcfRecord>& recs, const vtx_clusters& cl,
+                           const std::vector<std::string>& names)
 {
     FILE* f = fopen(path.c_str(), "wb");
     if (!f) return false;
     fputs("variant\tused", f);
-    for (uint32_t j = 0; j < cl.k; ++j) fprintf(f, "\tref_C%u\talt_C%u", j, j);
+    for (uint32_t j = 0; j < cl.k; ++j) fprintf(f, "\tref_%s\talt_%s", names[j].c_str(), names[j].c_str());
     fputc('\n', f);
     const double w = double(vtx::clusters::kW);
     for (size_t v = 0; v < recs.size(); ++v) {
@@ -786,14 +861,16 @@ int main(int argc, char** argv)
     // donor list or sample header is refused first
     std::vector<VcfRecord> recs;
     const bool with_donors = !o.out_donors.empty();
-    const bool with_ambient = !o.ambient_rna.empty();      // the donors are scored once, after the finish, over the result
+    const bool with_ambient = with_donors && !o.ambient_rna.empty();      // the donors are scored once, after the finish, over the result
     const bool with_matches = !o.out_cluster_matches.empty();
     const bool with_cluster_gt = with_matches || !o.out_cluster_genotypes.empty();
-    DonorTable donors;
+    const bool with_known = !o.known.empty();
+    DonorTable donors, known;
     VcfGenotypes gts;
-    if (with_donors || with_matches) {
+    if (with_donors || with_matches || with_known) {
         if (!read_vcf(o.vcf, &recs, &err, &gts)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
         if (with_donors && !select_donors(o.donors, gts, recs, &donors, &err)) { fprintf(stderr, "error: %s\n", err.c_str()); return 1; }
+        if (with_known && !select_known(o.known, gts, recs, &known, &err)) { fprintf(stderr, "error: %s\n", err.c_str()); return 1; }
         if (with_matches && (gts.samples.empty() || gts.samples.size() > vtx::cluster_gt::kMaxSamples)) {
             fprintf(stderr, "error: --out-cluster-matches needs 1 to %u sample columns in the VCF, not %zu\n", vtx::cluster_gt::kMaxSamples,
                     gts.samples.size());
@@ -835,7 +912,7 @@ int main(int argc, char** argv)
         }
     }
 
-    if (!with_donors && !with_matches && !read_vcf(o.vcf, &recs, &err)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
+    if (!with_donors && !with_matches && !with_known && !read_vcf(o.vcf, &recs, &err)) { printf("Vartrix error.\nError: %s\n", err.c_str()); return 1; }
     if (recs.empty()) LOG_ERR("Warning! Zero variants found in input VCF. Output matrices will be by definition empty but will still be generated.");
     LOG_INFO("Initialized a %zu variants x %zu cell barcodes matrix", recs.size(), bcs.keys.size());
     LOG_INFO("[%.3f s] inputs parsed", now_s());
@@ -1239,20 +1316,32 @@ int main(int argc, char** argv)
         validate_output_path(o.out_clusters);
         if (!o.out_cluster_alleles.empty()) validate_output_path(o.out_cluster_alleles);
         const vtx_cluster_params cp{ o.clusters, o.cluster_restarts, o.cluster_seed };
+        const uint32_t J = uint32_t(known.names.size());
+        const int32_t pin_m = o.ambient_rna.empty() ? 0 : o.ambient_permille;       // --known-donors: rho is given, 0 by default
+        const vtx_cluster_pinned_params pp{ o.clusters, o.cluster_restarts, o.cluster_seed, J, 0.01, pin_m };
         vtx_clusters cl{};
-        if (vtx_cluster_cells(ctx, res.n, res.row, res.col, res.ref_cnt, res.alt_cnt, recs.size(), uint32_t(bcs.keys.size()), &cp, &cl) != VTX_OK) {
+        const int crc = with_known ? vtx_cluster_cells_pinned(ctx, res.n, res.row, res.col, res.ref_cnt, res.alt_cnt, recs.size(),
+                                                              uint32_t(bcs.keys.size()), known.dosage.data(), &pp, &cl)
+                                   : vtx_cluster_cells(ctx, res.n, res.row, res.col, res.ref_cnt, res.alt_cnt, recs.size(), uint32_t(bcs.keys.size()), &cp, &cl);
+        if (crc != VTX_OK) {
             printf("Vartrix error.\nError: %s\n", vtx_last_error(ctx)); rc = 1;
         } else {
-            std::vector<std::string> names;
-            for (uint32_t j = 0; j < cl.k; ++j) names.push_back("C" + std::to_string(j));
+            std::vector<std::string> names = known.names;             // the known samples, then the free clusters
+            for (uint32_t j = 0; j < cl.k - J; ++j) names.push_back("C" + std::to_string(j));
             const std::vector<int64_t> ll(cl.ll, cl.ll + size_t(cl.n_cols) * cl.n_hyp);
             const std::vector<uint64_t> cnt(cl.counts, cl.counts + size_t(cl.n_cols) * 3);
             uint64_t calls[3] = { 0, 0, 0 };
             if (!write_donors(o.out_clusters, bcs.keys, names, ll, cnt, calls)) { LOG_ERR("error writing cluster file"); rc = 1; }
-            if (!o.out_cluster_alleles.empty() && !write_cluster_alleles(o.out_cluster_alleles, recs, cl)) { LOG_ERR("error writing cluster allele file"); rc = 1; }
-            LOG_INFO("Clusters: %u, restarts %u, seed %llu; best restart %u after %u iterations; rows used: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
-                     cl.k, o.cluster_restarts, (unsigned long long)o.cluster_seed, cl.best_restart, cl.restart_iters[cl.best_restart],
-                     (unsigned long long)cl.rows_used, recs.size(), (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
+            if (!o.out_cluster_alleles.empty() && !write_cluster_alleles(o.out_cluster_alleles, recs, cl, names)) { LOG_ERR("error writing cluster allele file"); rc = 1; }
+            if (with_known)
+                LOG_INFO("Clusters with known donors: %u, known %s, ambient RNA %.3f (given), restarts %u, seed %llu; best restart %u after %u iterations; rows used: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
+                         cl.k, o.known_donors.c_str(), pin_m / 1000.0, o.cluster_restarts, (unsigned long long)o.cluster_seed, cl.best_restart,
+                         cl.restart_iters[cl.best_restart], (unsigned long long)cl.rows_used, recs.size(), (unsigned long long)calls[0],
+                         (unsigned long long)calls[1], (unsigned long long)calls[2]);
+            else
+                LOG_INFO("Clusters: %u, restarts %u, seed %llu; best restart %u after %u iterations; rows used: %llu of %zu; cells: %llu singlet, %llu doublet, %llu unassigned",
+                         cl.k, o.cluster_restarts, (unsigned long long)o.cluster_seed, cl.best_restart, cl.restart_iters[cl.best_restart],
+                         (unsigned long long)cl.rows_used, recs.size(), (unsigned long long)calls[0], (unsigned long long)calls[1], (unsigned long long)calls[2]);
             if (with_cluster_gt && cluster_genotypes(o, ctx, res, recs, gts, cl) != 0) rc = 1;
             if (!o.out_cluster_calls.empty() && cluster_calls(o, ctx, res, recs, bcs.keys, cl) != 0) rc = 1;
         }

@@ -12,6 +12,7 @@
 #include "vtx_ambient.cuh"
 #include "vtx_cluster_gt.cuh"
 #include "vtx_cluster_refine.cuh"
+#include "vtx_cluster_pinned.cuh"
 
 #include <nvtx3/nvToolsExt.h>     // header-only; ranges cost nothing unless a profiler (nsys / ncu --nvtx) is attached
 
@@ -180,6 +181,8 @@ struct vtx_ctx {
     std::vector<uint32_t> h_cr_label, h_cr_pl;
     std::vector<uint8_t> h_cr_gt;
     std::vector<vtx_cluster_calls_round> h_cr_rounds;
+    // vtx_cluster_cells_pinned: the pinned samples' dosage (everything else is vtx_cluster_cells', the row sums in am_sums)
+    DBuf cp_dos;
     HostBuf h_stage;                                 // scalars read back between the staging phases
     uint32_t bc_cap = 0, n_barcodes = 0;
     bool have_barcodes = false;
@@ -1677,26 +1680,30 @@ int vtx_donor_ll_get(vtx_ctx* ctx, const int64_t** ll, const uint64_t** counts, 
     return VTX_OK;
 }
 
-int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
-                      const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params, vtx_clusters* out)
+// The pinned samples of vtx_cluster_cells_pinned (DESIGN.md §5k); J = 0 is vtx_cluster_cells
+struct PinSpec {
+    uint32_t J = 0, m = 0;
+    double error_rate = 0;
+    const uint8_t* dosage = nullptr;        // host [n_rows][J]
+};
+
+// vtx_cluster_cells and vtx_cluster_cells_pinned: §5g's EM and scoring; with pins, the J pinned clusters' logs are overwritten
+// after the init and after every M-step, the pinned clusters keep their indices, and the scoring takes their pinned theta
+static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                             const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params,
+                             const PinSpec& pin, vtx_clusters* out)
 {
     using namespace clusters;
-    if (!ctx || !params || !out) return VTX_E_INVALID;
-    *out = vtx_clusters{};
-    if (!ctx->finished || ctx->gather_pending)
-        return set_err(ctx, VTX_E_STATE, "vtx_cluster_cells: submits are unfinished (call vtx_finish / vtx_finish_device first)");
-    const uint32_t K = params->k, R = params->restarts;
-    if (K < kMinK || K > kMaxK) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: k = %u; 2 to 32 clusters are supported", K);
-    if (R < 1 || R > kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: %u restarts; 1 to 64 are supported", R);
-    if (n && (!row || !col || !ref_cnt || !alt_cnt)) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: an entry array is NULL");
+    const uint32_t K = params->k, R = params->restarts, J = pin.J;
+    if (n && (!row || !col || !ref_cnt || !alt_cnt)) return set_err(ctx, VTX_E_INVALID, "%s: an entry array is NULL", fn);
     if (n > 0xFFFFFFFFull || n_rows > 0xFFFFFFFFull)
-        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: %llu entries over %llu rows; both must be below 2^32",
+        return set_err(ctx, VTX_E_INVALID, "%s: %llu entries over %llu rows; both must be below 2^32", fn,
                        (unsigned long long)n, (unsigned long long)n_rows);
     const uint32_t H = donors::n_hyp(K);
     // device memory, before any host table of n_rows entries: the by-row entries (16 B) and their by-cell copy (12 B), the
-    // weights, the tables, the final sums and the outputs
+    // weights, the tables, the final sums and the outputs; with pins, the dosage and the row sums
     const double need = double(n) * 28 + double(n_rows) * (5 + 16.0 * K) + double(n_cols) * (12 + 24 + 8.0 * H) +
-                        double(R) * n_cols * K * 4 + double(R) * double(n_rows) * K * 8;
+                        double(R) * n_cols * K * 4 + double(R) * double(n_rows) * K * 8 + (J ? double(n_rows) * (J + 16) : 0.0);
     {
         CK(cudaSetDevice(ctx->device));
         size_t free_b = 0, total_b = 0;
@@ -1706,16 +1713,22 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
                          &ctx->cl_cell_count, &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_la, &ctx->cl_lr,
                          &ctx->cl_w, &ctx->cl_flags, &ctx->cl_A, &ctx->cl_T, &ctx->cl_ll, &ctx->cl_cnt })
             held += b->cap;
+        if (J) held += ctx->cp_dos.cap + ctx->am_sums.cap;
         if (need > double(free_b) + double(held))
-            return set_err(ctx, VTX_E_NOMEM, "vtx_cluster_cells needs %.0f MB of device memory, %.0f MB are free", need * 1e-6,
+            return set_err(ctx, VTX_E_NOMEM, "%s needs %.0f MB of device memory, %.0f MB are free", fn, need * 1e-6,
                            (double(free_b) + double(held)) * 1e-6);
     }
+    const size_t n_dos = size_t(n_rows) * J;
+    for (size_t i = 0; i < n_dos; ++i)
+        if (pin.dosage[i] > 2 && pin.dosage[i] != donors::kMissing)
+            return set_err(ctx, VTX_E_INVALID, "%s: dosage %u at row %zu, sample %zu (0, 1, 2 or VTX_GT_MISSING)", fn,
+                           unsigned(pin.dosage[i]), i / J, i % J);
     // validate the entries in one pass; rows are contiguous, so the per-row counts need no table
     std::vector<uint32_t> row_start(size_t(n_rows) + 1, 0);
     ctx->h_cl_used.assign(size_t(n_rows), 0);
     std::vector<uint32_t> used_rows;
     const uint64_t kMaxMolecules = ((1ull << 53) - (1ull << 17)) >> 16;     // molecules x 2^16 + 2^17 stays below 2^53
-    int vrc = validate_entries(ctx, "vtx_cluster_cells", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxMolecules,
+    int vrc = validate_entries(ctx, fn, n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxMolecules,
                                "its weighted sums would not be exact", [&](uint32_t v, uint64_t i0, uint64_t i1, uint64_t) {
         uint32_t with_ref = 0, with_alt = 0;
         for (uint64_t i = i0; i < i1; ++i) { with_ref += ref_cnt[i] > 0; with_alt += alt_cnt[i] > 0; }
@@ -1768,8 +1781,35 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
     CK(cudaGetLastError());
     const CellEntries ce{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
 
-    // the EM: every active restart in the same launches; the host reads the restarts' flags and scores once per iteration
+    // the pinned samples' dosage and the row sums A_v, T_v over every entry (§5h's kernel)
+    cluster_pinned::Pins pins{};
+    if (J) {
+        ENS(ctx->cp_dos, n_dos + 8);
+        ENS(ctx->am_sums, size_t(n_rows) * 16 + 16);
+        if (n_dos) CK(cudaMemcpyAsync(ctx->cp_dos.p, pin.dosage, n_dos, cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(ctx->am_sums.p, 0, size_t(n_rows) * 16, st));
+        pins.J = J; pins.m = pin.m; pins.fr = ambient::fractions(pin.error_rate);
+        pins.dos = P<uint8_t>(ctx->cp_dos);
+        pins.rowA = P<unsigned long long>(ctx->am_sums);
+        pins.rowT = pins.rowA + n_rows;
+        if (n) {
+            ambient::vtx_k_am_rowsum<<<egrid, ambient::kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a),
+                                                                             P<unsigned long long>(ctx->am_sums), P<unsigned long long>(ctx->am_sums) + n_rows);
+            CK(cudaGetLastError());
+        }
+    }
     const uint32_t n_used = uint32_t(used_rows.size());
+    // the pinned logs of the active restarts over §5g's tables
+    auto pin_logs = [&](const Active& a) -> int {
+        if (!J || !n_used || !a.n) return VTX_OK;
+        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(a.n) * n_used * J, cluster_pinned::kCpThreads), unsigned(ctx->n_sm) * 16));
+        cluster_pinned::vtx_k_cp_pin<<<g, cluster_pinned::kCpThreads, 0, st>>>(a, pins, n_used, P<uint32_t>(ctx->cl_used_rows), K, n_rows,
+                                                                             P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr));
+        CK(cudaGetLastError());
+        return VTX_OK;
+    };
+
+    // the EM: every active restart in the same launches; the host reads the restarts' flags and scores once per iteration
     if (n_used) {
         const unsigned igrid = std::max(1u, std::min(blocks_for(uint64_t(R) * n_used * K, kClThreads), unsigned(ctx->n_sm) * 16));
         vtx_k_cl_init<<<igrid, kClThreads, 0, st>>>(params->seed, R, K, n_used, P<uint32_t>(ctx->cl_used_rows), n_rows,
@@ -1781,6 +1821,8 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
     ctx->h_cl_iters.assign(R, 0);
     Active act{};
     for (uint32_t s = 0; s < R; ++s) act.s[act.n++] = uint8_t(s);
+    rc = pin_logs(act);
+    if (rc) return rc;
     uint32_t* d_changed = P<uint32_t>(ctx->cl_flags);
     unsigned long long* d_score = reinterpret_cast<unsigned long long*>(d_changed + R + (R & 1));
     std::vector<uint32_t> h_flags(flag_bytes / 4);
@@ -1809,20 +1851,22 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
                                                      P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a),
                                                      P<uint32_t>(ctx->cl_w), n_cols, n_rows, K, P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr));
             CK(cudaGetLastError());
+            rc = pin_logs(act);
+            if (rc) return rc;
         }
     }
     uint32_t best = 0;
     for (uint32_t s = 1; s < R; ++s)
         if (ctx->h_cl_score[s] > ctx->h_cl_score[best]) best = s;
 
-    // canonical order: the best restart's clusters by sum_c W_ck, descending, ties by EM index
+    // canonical order: the best restart's clusters by sum_c W_ck, descending, ties by EM index (the pinned clusters keep theirs)
     std::vector<uint32_t> w_best(size_t(n_cols) * K);
     if (n_cols) CK(cudaMemcpy(w_best.data(), P<uint32_t>(ctx->cl_w) + size_t(best) * n_cols * K, w_best.size() * 4, cudaMemcpyDeviceToHost));
     std::vector<uint64_t> tot(K, 0);
     for (size_t i = 0; i < w_best.size(); ++i) tot[i % K] += w_best[i];
     std::vector<uint32_t> order(K);
     for (uint32_t k = 0; k < K; ++k) order[k] = k;
-    std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return tot[x] > tot[y]; });
+    std::stable_sort(order.begin() + J, order.end(), [&](uint32_t x, uint32_t y) { return tot[x] > tot[y]; });
     Perm perm{};
     for (uint32_t j = 0; j < K; ++j) perm.k[j] = uint8_t(order[j]);
 
@@ -1840,7 +1884,15 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
         const int64_t* T = P<int64_t>(ctx->cl_T);
         int64_t* ll = P<int64_t>(ctx->cl_ll);
         uint64_t* cnt = P<uint64_t>(ctx->cl_cnt);
-        if (H <= 32) vtx_k_cl_score<1><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
+        using cluster_pinned::vtx_k_cl_score_pinned;
+        if (J) {
+            if (H <= 32) vtx_k_cl_score_pinned<1><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
+            else if (H <= 64) vtx_k_cl_score_pinned<2><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
+            else if (H <= 160) vtx_k_cl_score_pinned<5><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
+            else if (H <= 288) vtx_k_cl_score_pinned<9><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
+            else vtx_k_cl_score_pinned<17><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
+        }
+        else if (H <= 32) vtx_k_cl_score<1><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
         else if (H <= 64) vtx_k_cl_score<2><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
         else if (H <= 160) vtx_k_cl_score<5><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
         else if (H <= 288) vtx_k_cl_score<9><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
@@ -1867,6 +1919,45 @@ int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint3
     out->alt_w = ctx->h_cl_A.data(); out->depth_w = ctx->h_cl_T.data();
     out->restart_score = ctx->h_cl_score.data(); out->restart_iters = ctx->h_cl_iters.data();
     return VTX_OK;
+}
+
+int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                      const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params, vtx_clusters* out)
+{
+    using namespace clusters;
+    if (!ctx || !params || !out) return VTX_E_INVALID;
+    *out = vtx_clusters{};
+    if (!ctx->finished || ctx->gather_pending)
+        return set_err(ctx, VTX_E_STATE, "vtx_cluster_cells: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const uint32_t K = params->k, R = params->restarts;
+    if (K < kMinK || K > kMaxK) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: k = %u; 2 to 32 clusters are supported", K);
+    if (R < 1 || R > kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: %u restarts; 1 to 64 are supported", R);
+    return cluster_cells_run(ctx, "vtx_cluster_cells", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, params, PinSpec{}, out);
+}
+
+int vtx_cluster_cells_pinned(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
+                             const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const uint8_t* dosage,
+                             const vtx_cluster_pinned_params* params, vtx_clusters* out)
+{
+    using namespace clusters;
+    if (!ctx || !params || !out) return VTX_E_INVALID;
+    *out = vtx_clusters{};
+    const char* fn = "vtx_cluster_cells_pinned";
+    if (!ctx->finished || ctx->gather_pending)
+        return set_err(ctx, VTX_E_STATE, "%s: submits are unfinished (call vtx_finish / vtx_finish_device first)", fn);
+    const uint32_t K = params->k, R = params->restarts, J = params->n_pinned;
+    if (K < kMinK || K > kMaxK) return set_err(ctx, VTX_E_INVALID, "%s: k = %u; 2 to 32 clusters are supported", fn, K);
+    if (R < 1 || R > kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "%s: %u restarts; 1 to 64 are supported", fn, R);
+    if (J < 1 || J >= K) return set_err(ctx, VTX_E_INVALID, "%s: %u pinned samples; 1 to k - 1 = %u are supported", fn, J, K - 1);
+    if (!dosage) return set_err(ctx, VTX_E_INVALID, "%s: dosage is NULL", fn);
+    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
+        return set_err(ctx, VTX_E_INVALID, "%s: error rate %g outside [1e-6, 0.25]", fn, params->error_rate);
+    if (params->rho_permille < 0 || params->rho_permille > ambient::kMaxPermille)
+        return set_err(ctx, VTX_E_INVALID, "%s: rho_permille %d; 0 to 500", fn, params->rho_permille);
+    const vtx_cluster_params cp{ K, R, params->seed };
+    PinSpec pin;
+    pin.J = J; pin.m = uint32_t(params->rho_permille); pin.error_rate = params->error_rate; pin.dosage = dosage;
+    return cluster_cells_run(ctx, fn, n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, &cp, pin, out);
 }
 
 int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,

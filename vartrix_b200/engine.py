@@ -370,6 +370,21 @@ def _np_from(ptr, n, dt, copy=True):
     return a.copy() if copy else a
 
 
+def _clusters_dict(out, restarts: int) -> dict:
+    """NumPy copies of a vtx_clusters (library-owned memory that the next clustering call reuses)"""
+    def arr(ptr, count, dtype, shape):
+        if count == 0:
+            return np.zeros(shape, dtype)
+        return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
+    nc, nh, nr, kk = int(out.n_cols), int(out.n_hyp), int(out.n_rows), int(out.k)
+    return dict(k=kk, n_hyp=nh, best_restart=int(out.best_restart), rows_used=int(out.rows_used),
+                ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
+                row_used=arr(out.row_used, nr, np.uint8, (nr,)), alt_w=arr(out.alt_w, nr * kk, np.int64, (nr, kk)),
+                depth_w=arr(out.depth_w, nr * kk, np.int64, (nr, kk)),
+                restart_score=arr(out.restart_score, restarts, np.int64, (restarts,)),
+                restart_iters=arr(out.restart_iters, restarts, np.uint32, (restarts,)))
+
+
 class Engine:
     """One engine context = one GPU (vtx_ctx).  Mirrors the role of the rayon pool + merge loop."""
 
@@ -631,18 +646,29 @@ class Engine:
         p = _capi.ClusterParams(int(k), int(restarts), int(seed) & 0xFFFFFFFFFFFFFFFF)
         ptr = [x.ctypes.data if n else None for x in arrs]
         self._ck(self._L.vtx_cluster_cells(self._h, n, *ptr, int(n_rows), int(n_cols), C.byref(p), C.byref(out)), "vtx_cluster_cells")
+        return _clusters_dict(out, int(restarts))
 
-        def arr(ptr, count, dtype, shape):
-            if count == 0:
-                return np.zeros(shape, dtype)
-            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
-        nc, nh, nr, kk = int(out.n_cols), int(out.n_hyp), int(out.n_rows), int(out.k)
-        return dict(k=kk, n_hyp=nh, best_restart=int(out.best_restart), rows_used=int(out.rows_used),
-                    ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
-                    row_used=arr(out.row_used, nr, np.uint8, (nr,)), alt_w=arr(out.alt_w, nr * kk, np.int64, (nr, kk)),
-                    depth_w=arr(out.depth_w, nr * kk, np.int64, (nr, kk)),
-                    restart_score=arr(out.restart_score, int(restarts), np.int64, (int(restarts),)),
-                    restart_iters=arr(out.restart_iters, int(restarts), np.uint32, (int(restarts),)))
+    def cluster_cells_pinned(self, row, col, ref, alt, n_rows: int, n_cols: int, k: int, dosage, rho_permille: int = 0,
+                             error_rate: float = 0.01, restarts: int = 8, seed: int = 0) -> dict:
+        """Clustering with the first J clusters pinned to known genotypes (vtx_cluster_cells_pinned, include/vartrix_b200.h;
+        DESIGN.md §5k): count entries as cluster_cells takes them, dosage uint8[n_rows, J] (0, 1, 2 or GT_MISSING) of the J
+        genotyped samples, 1 <= J <= k - 1, and the ambient fraction rho_permille / 1000 (an integer m in 0..500).  -> the dict
+        cluster_cells returns; clusters 0 .. J - 1 are the samples in dosage's column order, J .. k - 1 the free clusters."""
+        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
+        n = len(arrs[0])
+        if any(len(x) != n for x in arrs):
+            raise ValueError("row, col, ref and alt must have the same length")
+        g = np.ascontiguousarray(dosage, dtype=np.uint8)
+        if g.ndim != 2 or g.shape[0] != int(n_rows):
+            raise ValueError(f"dosage must be a [n_rows, samples] array, not shape {g.shape}")
+        if isinstance(rho_permille, (bool, np.bool_)) or not isinstance(rho_permille, (int, np.integer)):
+            raise TypeError(f"rho_permille must be an integer number of thousandths, not {rho_permille!r}")
+        out = _capi.Clusters()
+        p = _capi.ClusterPinnedParams(int(k), int(restarts), int(seed) & 0xFFFFFFFFFFFFFFFF, g.shape[1], float(error_rate), int(rho_permille))
+        ptr = [x.ctypes.data if n else None for x in arrs]
+        self._ck(self._L.vtx_cluster_cells_pinned(self._h, n, *ptr, int(n_rows), int(n_cols), g.ctypes.data, C.byref(p), C.byref(out)),
+                 "vtx_cluster_cells_pinned")
+        return _clusters_dict(out, int(restarts))
 
     def donors_ambient(self, row, col, ref, alt, n_rows: int, n_cols: int, dosage, error_rate: float = 0.01, rho_permille=None,
                        grid_batch: int = 0) -> dict:
