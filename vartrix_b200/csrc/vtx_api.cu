@@ -22,8 +22,10 @@
 #include <cstddef>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 using namespace vtx;
@@ -279,6 +281,23 @@ TimeRec* new_trec(vtx_ctx* ctx)
 }
 
 inline unsigned blocks_for(uint64_t n, unsigned threads) { return unsigned((n + threads - 1) / threads); }
+
+// the grid of a grid-stride kernel over `work` threads: at most per_sm CTAs per SM, at least one
+inline unsigned grid_for(const vtx_ctx* ctx, uint64_t work, unsigned threads, unsigned per_sm = 16)
+{
+    return std::max(1u, std::min(blocks_for(work, threads), unsigned(ctx->n_sm) * per_sm));
+}
+
+// launch(std::integral_constant<int, KH>{}) for a warp-per-cell kernel over H hypotheses, lane l owning hypotheses l + 32j,
+// j < KH: the smallest of the instantiations KH = 1, 2, 5, 9, 17 with 32 KH >= H
+template <typename Launch> void by_kh(uint32_t H, Launch launch)
+{
+    if (H <= 32) launch(std::integral_constant<int, 1>{});
+    else if (H <= 64) launch(std::integral_constant<int, 2>{});
+    else if (H <= 160) launch(std::integral_constant<int, 5>{});
+    else if (H <= 288) launch(std::integral_constant<int, 9>{});
+    else launch(std::integral_constant<int, 17>{});
+}
 
 // exclusive scan on stream `st` with block sums in `sums`: out has n + 1 entries
 int scan_u32(vtx_ctx* ctx, cudaStream_t st, DBuf& sums, const uint32_t* in, uint64_t n, uint32_t* out, uint64_t* launches)
@@ -586,7 +605,7 @@ int launch_donors(vtx_ctx* ctx, const DevBatch& b, uint32_t n_slots_ub, const ui
     int64_t* ll = P<int64_t>(ctx->donor_acc);
     uint64_t* cnt = reinterpret_cast<uint64_t*>(ll + size_t(nc) * H);
     unsigned long long* bad = reinterpret_cast<unsigned long long*>(cnt + size_t(nc) * 3);
-    const unsigned grid = std::max(1u, std::min(blocks_for(std::max<uint64_t>(n_slots_ub, b.n_loci), kDonorThreads), unsigned(ctx->n_sm) * 16));
+    const unsigned grid = grid_for(ctx, std::max<uint64_t>(n_slots_ub, b.n_loci), kDonorThreads);
     ENS(ctx->donor_count, (size_t(nc) + 1) * 4);
     CK(cudaMemsetAsync(ctx->donor_count.p, 0, size_t(nc) * 4, st));
     vtx_k_donor_count<<<grid, kDonorThreads, 0, st>>>(in, n_slots_ub, n_slots, b.n_loci, P<uint32_t>(ctx->donor_count), bad);
@@ -600,15 +619,11 @@ int launch_donors(vtx_ctx* ctx, const DevBatch& b, uint32_t n_slots_ub, const ui
     CK(cudaMemsetAsync(ctx->donor_count.p, 0, size_t(nc) * 4, st));
     vtx_k_donor_scatter<<<grid, kDonorThreads, 0, st>>>(in, n_slots_ub, n_slots, P<uint32_t>(ctx->donor_start),
                                                         P<uint32_t>(ctx->donor_count), P<uint32_t>(ctx->donor_list));
-    // one warp per column; KH = ceil(H / 32) accumulators per lane, from the instantiations below
-    const unsigned ll_grid = std::max(1u, std::min(blocks_for(uint64_t(nc) * 32, kDonorThreads), unsigned(ctx->n_sm) * 8));
+    // one warp per column
+    const unsigned ll_grid = grid_for(ctx, uint64_t(nc) * 32, kDonorThreads, 8);
     const uint32_t* cs = P<uint32_t>(ctx->donor_start);
     const uint32_t* lst = P<uint32_t>(ctx->donor_list);
-    if (H <= 32) vtx_k_donor_ll<1><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
-    else if (H <= 64) vtx_k_donor_ll<2><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
-    else if (H <= 160) vtx_k_donor_ll<5><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
-    else if (H <= 288) vtx_k_donor_ll<9><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
-    else vtx_k_donor_ll<17><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt);
+    by_kh(H, [&](auto kh) { vtx_k_donor_ll<decltype(kh)::value><<<ll_grid, kDonorThreads, 0, st>>>(in, cs, lst, ll, cnt); });
     CK(cudaGetLastError());
     *launches += 2;
     return VTX_OK;
@@ -1171,7 +1186,7 @@ int cg_fit_device(vtx_ctx* ctx, const ambient::Fractions& fr, uint32_t K, int32_
             for (uint32_t b = 0; b < bt.n; ++b) bt.m[b] = list[o + b];
             CK(cudaMemsetAsync(d_J, 0, size_t(ambient::kMaxBatch) * 8, st));
             if (n_fit) {
-                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_fit * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
+                const unsigned g = grid_for(ctx, uint64_t(bt.n) * n_fit * 32, kCgThreads);
                 vtx_k_cg_fit<<<g, kCgThreads, 0, st>>>(bt, fr, K, n_fit, d_fit, d_rowA, d_rowT, d_A, d_T, d_J);
                 CK(cudaGetLastError());
             }
@@ -1187,12 +1202,145 @@ int cg_fit_device(vtx_ctx* ctx, const ambient::Fractions& fr, uint32_t K, int32_
     else { ms.assign(1, uint16_t(*chosen)); rc = evaluate(ms); }
     if (rc) return rc;
     if (n_t) {
-        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_t) * 32, kCgThreads), unsigned(ctx->n_sm) * 16));
+        const unsigned g = grid_for(ctx, uint64_t(n_t) * 32, kCgThreads);
         vtx_k_cg_call<<<g, kCgThreads, 0, st>>>(*chosen, fr, K, n_t, d_rowA, d_rowT, d_A, d_T, P<int64_t>(ctx->cg_ll), P<uint8_t>(ctx->cg_gt),
                                                  P<uint32_t>(ctx->cg_pl));
         CK(cudaGetLastError());
     }
     return VTX_OK;
+}
+
+// ---- the post-passes' shared intake (vtx_cluster_cells*, vtx_donors_ambient, vtx_cluster_genotypes, vtx_cluster_refine) ----
+
+int check_finished(vtx_ctx* ctx, const char* fn)
+{
+    if (!ctx->finished || ctx->gather_pending)
+        return set_err(ctx, VTX_E_STATE, "%s: submits are unfinished (call vtx_finish / vtx_finish_device first)", fn);
+    return VTX_OK;
+}
+
+int check_error_rate(vtx_ctx* ctx, const char* fn, double error_rate)
+{
+    if (!(error_rate >= 1e-6 && error_rate <= 0.25))
+        return set_err(ctx, VTX_E_INVALID, "%s: error rate %g outside [1e-6, 0.25]", fn, error_rate);
+    return VTX_OK;
+}
+
+int check_k(vtx_ctx* ctx, const char* fn, uint32_t K)
+{
+    if (K < clusters::kMinK || K > clusters::kMaxK) return set_err(ctx, VTX_E_INVALID, "%s: k = %u; 2 to 32 clusters are supported", fn, K);
+    return VTX_OK;
+}
+
+// one row of a dosage table, g[width]: 0, 1, 2 or VTX_GT_MISSING; `noun` names a column ("donor", "sample")
+int check_dosage_row(vtx_ctx* ctx, const char* fn, const uint8_t* g, uint32_t width, uint64_t row, const char* noun)
+{
+    for (uint32_t s = 0; s < width; ++s)
+        if (g[s] > 2 && g[s] != donors::kMissing)
+            return set_err(ctx, VTX_E_INVALID, "%s: dosage %u at row %llu, %s %u (0, 1, 2 or VTX_GT_MISSING)", fn, unsigned(g[s]),
+                           (unsigned long long)row, noun, s);
+    return VTX_OK;
+}
+
+// row v of a clustering's sums, alt_w / depth_w [K], within §5i's bounds; *total is the depth_w sum over the rows so far
+int check_sums_row(vtx_ctx* ctx, const char* fn, const int64_t* alt_w, const int64_t* depth_w, uint32_t K, uint64_t v, uint64_t* total)
+{
+    for (uint32_t k = 0; k < K; ++k) {
+        const int64_t a = alt_w[k], t = depth_w[k];
+        if (a < 0 || a > t || t > cluster_gt::kMaxDepthW)
+            return set_err(ctx, VTX_E_INVALID, "%s: row %llu, cluster %u: alt_w %lld, depth_w %lld (0 <= alt_w <= depth_w <= 2^51)", fn,
+                           (unsigned long long)v, k, (long long)a, (long long)t);
+        *total += uint64_t(t);
+        if (*total > cluster_gt::kMaxTotalDepthW)
+            return set_err(ctx, VTX_E_INVALID, "%s: depth_w sums to more than 2^51 over the rows; the fit's int64 sums would not be exact", fn);
+    }
+    return VTX_OK;
+}
+
+// Refuses a call that needs `need` bytes of device memory when fewer are available: free memory plus the capacity of `held`,
+// the buffers the call ensures (ensure frees them before it grows them; a buffer the call does not ensure stays allocated, so a
+// null entry counts nothing).  *avail gets the available bytes.
+int check_free(vtx_ctx* ctx, const char* fn, double need, std::initializer_list<const DBuf*> held, double* avail = nullptr)
+{
+    CK(cudaSetDevice(ctx->device));
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    size_t held_b = 0;
+    for (const DBuf* b : held) held_b += b ? b->cap : 0;
+    const double a = double(free_b) + double(held_b);
+    if (avail) *avail = a;
+    if (need > a) return set_err(ctx, VTX_E_NOMEM, "%s needs %.0f MB of device memory, %.0f MB are free", fn, need * 1e-6, a * 1e-6);
+    return VTX_OK;
+}
+
+// Uploads n count entries to cl_row / cl_col / cl_r / cl_a and groups by cell those at rows flagged in cl_used (already on the
+// stream) with r + a > 0: §5g's count, scan and scatter into cl_cell_start and cl_c_*
+int cell_entries(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt, const uint32_t* alt_cnt,
+                 uint32_t n_cols, clusters::CellEntries* ce)
+{
+    using namespace clusters;
+    cudaStream_t st = ctx->stream;
+    const size_t nb = size_t(n) * 4 + 4;
+    ENS(ctx->cl_row, nb); ENS(ctx->cl_col, nb); ENS(ctx->cl_r, nb); ENS(ctx->cl_a, nb);
+    ENS(ctx->cl_c_row, nb); ENS(ctx->cl_c_r, nb); ENS(ctx->cl_c_a, nb);
+    ENS(ctx->cl_cell_count, (size_t(n_cols) + 1) * 4);
+    ENS(ctx->cl_cell_start, (size_t(n_cols) + 1) * 4);
+    if (n) {
+        CK(cudaMemcpyAsync(ctx->cl_row.p, row, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_r.p, ref_cnt, n * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ctx->cl_a.p, alt_cnt, n * 4, cudaMemcpyHostToDevice, st));
+    }
+    const uint32_t nn = uint32_t(n);
+    const unsigned grid = grid_for(ctx, n, kClThreads);
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    vtx_k_cl_count<<<grid, kClThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                 P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_count));
+    CK(cudaGetLastError());
+    const int rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->cl_cell_count), n_cols, P<uint32_t>(ctx->cl_cell_start), nullptr);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
+    vtx_k_cl_scatter<<<grid, kClThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
+                                                   P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_start),
+                                                   P<uint32_t>(ctx->cl_cell_count), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r),
+                                                   P<uint32_t>(ctx->cl_c_a));
+    CK(cudaGetLastError());
+    *ce = CellEntries{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
+    return VTX_OK;
+}
+
+// §5h's row sums A_v / T_v over the n uploaded entries, into am_sums: *d_A, *d_T [n_rows]
+int pool_row_sums(vtx_ctx* ctx, uint64_t n, uint64_t n_rows, const unsigned long long** d_A, const unsigned long long** d_T)
+{
+    using namespace ambient;
+    cudaStream_t st = ctx->stream;
+    ENS(ctx->am_sums, size_t(n_rows) * 16 + 16);
+    unsigned long long* sums = P<unsigned long long>(ctx->am_sums);
+    CK(cudaMemsetAsync(sums, 0, size_t(n_rows) * 16, st));
+    if (n) {
+        vtx_k_am_rowsum<<<grid_for(ctx, n, kAmThreads), kAmThreads, 0, st>>>(uint32_t(n), P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_r),
+                                                                             P<uint32_t>(ctx->cl_a), sums, sums + n_rows);
+        CK(cudaGetLastError());
+    }
+    *d_A = sums;
+    *d_T = sums + n_rows;
+    return VTX_OK;
+}
+
+// the evaluated m (ms, with obj and, if given, 3 calls per m) in ascending order into m_out / obj_out / calls_out
+void sort_grid(const std::vector<uint16_t>& ms, const std::vector<int64_t>& obj, const std::vector<uint64_t>* calls,
+               std::vector<uint16_t>& m_out, std::vector<int64_t>& obj_out, std::vector<uint64_t>* calls_out)
+{
+    std::vector<size_t> order(ms.size());
+    for (size_t i = 0; i < order.size(); ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](size_t x, size_t y) { return ms[x] < ms[y]; });
+    m_out.resize(ms.size()); obj_out.resize(ms.size());
+    if (calls_out) calls_out->resize(ms.size() * 3);
+    for (size_t i = 0; i < order.size(); ++i) {
+        m_out[i] = ms[order[i]];
+        obj_out[i] = obj[order[i]];
+        if (calls_out) for (int k = 0; k < 3; ++k) (*calls_out)[3 * i + k] = (*calls)[3 * order[i] + k];
+    }
 }
 
 }  // namespace
@@ -1643,16 +1791,14 @@ int vtx_set_donors(vtx_ctx* ctx, uint32_t n_donors, uint64_t n_rows, const uint8
     if (ctx->submitted) return set_err(ctx, VTX_E_STATE, "vtx_set_donors must be called before the first submit");
     if (n_donors < kMinDonors || n_donors > kMaxDonors)
         return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: %u donors; 2 to 32 are supported", n_donors);
-    if (!(error_rate >= 1e-6 && error_rate <= 0.25))
-        return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: error rate %g outside [1e-6, 0.25]", error_rate);
+    if (int rc = check_error_rate(ctx, "vtx_set_donors", error_rate)) return rc;
     if (n_rows && !dosage) return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: dosage is NULL");
     const size_t cells = size_t(n_rows) * n_donors;
     std::vector<uint8_t> usable(size_t(n_rows) + 1, 0);
-    for (size_t i = 0; i < cells; ++i)
-        if (dosage[i] > 2 && dosage[i] != kMissing)
-            return set_err(ctx, VTX_E_INVALID, "vtx_set_donors: dosage %u at row %zu, donor %zu (0, 1, 2 or VTX_GT_MISSING)",
-                           unsigned(dosage[i]), i / n_donors, i % n_donors);
-    for (uint64_t r = 0; r < n_rows; ++r) usable[r] = row_usable(dosage + size_t(r) * n_donors, n_donors) ? 1 : 0;
+    for (uint64_t r = 0; r < n_rows; ++r) {
+        if (int rc = check_dosage_row(ctx, "vtx_set_donors", dosage + size_t(r) * n_donors, n_donors, r, "donor")) return rc;
+        usable[r] = row_usable(dosage + size_t(r) * n_donors, n_donors) ? 1 : 0;
+    }
     CK(cudaSetDevice(ctx->device));
     ENS(ctx->donor_dosage, cells + 16);
     ENS(ctx->donor_usable, usable.size());
@@ -1704,49 +1850,33 @@ static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uin
     // weights, the tables, the final sums and the outputs; with pins, the dosage and the row sums
     const double need = double(n) * 28 + double(n_rows) * (5 + 16.0 * K) + double(n_cols) * (12 + 24 + 8.0 * H) +
                         double(R) * n_cols * K * 4 + double(R) * double(n_rows) * K * 8 + (J ? double(n_rows) * (J + 16) : 0.0);
-    {
-        CK(cudaSetDevice(ctx->device));
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        size_t held = 0;
-        for (DBuf* b : { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_used_rows, &ctx->cl_row_start,
-                         &ctx->cl_cell_count, &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_la, &ctx->cl_lr,
-                         &ctx->cl_w, &ctx->cl_flags, &ctx->cl_A, &ctx->cl_T, &ctx->cl_ll, &ctx->cl_cnt })
-            held += b->cap;
-        if (J) held += ctx->cp_dos.cap + ctx->am_sums.cap;
-        if (need > double(free_b) + double(held))
-            return set_err(ctx, VTX_E_NOMEM, "%s needs %.0f MB of device memory, %.0f MB are free", fn, need * 1e-6,
-                           (double(free_b) + double(held)) * 1e-6);
-    }
+    int rc = check_free(ctx, fn, need, { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_used_rows,
+                                         &ctx->cl_row_start, &ctx->cl_cell_count, &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r,
+                                         &ctx->cl_c_a, &ctx->cl_la, &ctx->cl_lr, &ctx->cl_w, &ctx->cl_flags, &ctx->cl_A, &ctx->cl_T,
+                                         &ctx->cl_ll, &ctx->cl_cnt, J ? &ctx->cp_dos : nullptr, J ? &ctx->am_sums : nullptr });
+    if (rc) return rc;
     const size_t n_dos = size_t(n_rows) * J;
-    for (size_t i = 0; i < n_dos; ++i)
-        if (pin.dosage[i] > 2 && pin.dosage[i] != donors::kMissing)
-            return set_err(ctx, VTX_E_INVALID, "%s: dosage %u at row %zu, sample %zu (0, 1, 2 or VTX_GT_MISSING)", fn,
-                           unsigned(pin.dosage[i]), i / J, i % J);
+    for (uint64_t v = 0; J && v < n_rows; ++v)
+        if ((rc = check_dosage_row(ctx, fn, pin.dosage + size_t(v) * J, J, v, "sample"))) return rc;
     // validate the entries in one pass; rows are contiguous, so the per-row counts need no table
     std::vector<uint32_t> row_start(size_t(n_rows) + 1, 0);
     ctx->h_cl_used.assign(size_t(n_rows), 0);
     std::vector<uint32_t> used_rows;
     const uint64_t kMaxMolecules = ((1ull << 53) - (1ull << 17)) >> 16;     // molecules x 2^16 + 2^17 stays below 2^53
-    int vrc = validate_entries(ctx, fn, n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxMolecules,
-                               "its weighted sums would not be exact", [&](uint32_t v, uint64_t i0, uint64_t i1, uint64_t) {
+    rc = validate_entries(ctx, fn, n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxMolecules,
+                          "its weighted sums would not be exact", [&](uint32_t v, uint64_t i0, uint64_t i1, uint64_t) {
         uint32_t with_ref = 0, with_alt = 0;
         for (uint64_t i = i0; i < i1; ++i) { with_ref += ref_cnt[i] > 0; with_alt += alt_cnt[i] > 0; }
         row_start[size_t(v) + 1] = uint32_t(i1 - i0);
         if (with_ref >= kMinCells && with_alt >= kMinCells) { ctx->h_cl_used[v] = 1; used_rows.push_back(v); }
     });
-    if (vrc) return vrc;
+    if (rc) return rc;
     for (uint64_t v = 0; v < n_rows; ++v) row_start[v + 1] += row_start[v];
 
     cudaStream_t st = ctx->stream;
-    const size_t nb = size_t(n) * 4 + 4;
-    ENS(ctx->cl_row, nb); ENS(ctx->cl_col, nb); ENS(ctx->cl_r, nb); ENS(ctx->cl_a, nb);
-    ENS(ctx->cl_c_row, nb); ENS(ctx->cl_c_r, nb); ENS(ctx->cl_c_a, nb);
     ENS(ctx->cl_used, size_t(n_rows) + 1);
     ENS(ctx->cl_used_rows, used_rows.size() * 4 + 4);
     ENS(ctx->cl_row_start, row_start.size() * 4);
-    ENS(ctx->cl_cell_count, (size_t(n_cols) + 1) * 4);
-    ENS(ctx->cl_cell_start, (size_t(n_cols) + 1) * 4);
     const size_t tab = size_t(R) * size_t(n_rows) * K * 4 + 4;
     ENS(ctx->cl_la, tab); ENS(ctx->cl_lr, tab);
     ENS(ctx->cl_w, size_t(R) * n_cols * K * 4 + 4);
@@ -1754,55 +1884,28 @@ static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uin
     ENS(ctx->cl_flags, flag_bytes);
     ENS(ctx->cl_A, size_t(n_rows) * K * 8 + 8); ENS(ctx->cl_T, size_t(n_rows) * K * 8 + 8);
     ENS(ctx->cl_ll, size_t(n_cols) * H * 8 + 8); ENS(ctx->cl_cnt, size_t(n_cols) * 24 + 8);
-    if (n) {
-        CK(cudaMemcpyAsync(ctx->cl_row.p, row, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_r.p, ref_cnt, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_a.p, alt_cnt, n * 4, cudaMemcpyHostToDevice, st));
-    }
     if (n_rows) CK(cudaMemcpyAsync(ctx->cl_used.p, ctx->h_cl_used.data(), n_rows, cudaMemcpyHostToDevice, st));
     if (!used_rows.empty()) CK(cudaMemcpyAsync(ctx->cl_used_rows.p, used_rows.data(), used_rows.size() * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->cl_row_start.p, row_start.data(), row_start.size() * 4, cudaMemcpyHostToDevice, st));
 
     // the by-cell index of the used entries
-    const uint32_t nn = uint32_t(n);
-    const unsigned egrid = std::max(1u, std::min(blocks_for(n, kClThreads), unsigned(ctx->n_sm) * 16));
-    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
-    vtx_k_cl_count<<<egrid, kClThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
-                                                  P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_count));
-    CK(cudaGetLastError());
-    int rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->cl_cell_count), n_cols, P<uint32_t>(ctx->cl_cell_start), nullptr);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
-    vtx_k_cl_scatter<<<egrid, kClThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
-                                                    P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_start),
-                                                    P<uint32_t>(ctx->cl_cell_count), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r),
-                                                    P<uint32_t>(ctx->cl_c_a));
-    CK(cudaGetLastError());
-    const CellEntries ce{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
+    CellEntries ce;
+    if ((rc = cell_entries(ctx, n, row, col, ref_cnt, alt_cnt, n_cols, &ce))) return rc;
 
     // the pinned samples' dosage and the row sums A_v, T_v over every entry (§5h's kernel)
     cluster_pinned::Pins pins{};
     if (J) {
         ENS(ctx->cp_dos, n_dos + 8);
-        ENS(ctx->am_sums, size_t(n_rows) * 16 + 16);
         if (n_dos) CK(cudaMemcpyAsync(ctx->cp_dos.p, pin.dosage, n_dos, cudaMemcpyHostToDevice, st));
-        CK(cudaMemsetAsync(ctx->am_sums.p, 0, size_t(n_rows) * 16, st));
+        if ((rc = pool_row_sums(ctx, n, n_rows, &pins.rowA, &pins.rowT))) return rc;
         pins.J = J; pins.m = pin.m; pins.fr = ambient::fractions(pin.error_rate);
         pins.dos = P<uint8_t>(ctx->cp_dos);
-        pins.rowA = P<unsigned long long>(ctx->am_sums);
-        pins.rowT = pins.rowA + n_rows;
-        if (n) {
-            ambient::vtx_k_am_rowsum<<<egrid, ambient::kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a),
-                                                                             P<unsigned long long>(ctx->am_sums), P<unsigned long long>(ctx->am_sums) + n_rows);
-            CK(cudaGetLastError());
-        }
     }
     const uint32_t n_used = uint32_t(used_rows.size());
     // the pinned logs of the active restarts over §5g's tables
     auto pin_logs = [&](const Active& a) -> int {
         if (!J || !n_used || !a.n) return VTX_OK;
-        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(a.n) * n_used * J, cluster_pinned::kCpThreads), unsigned(ctx->n_sm) * 16));
+        const unsigned g = grid_for(ctx, uint64_t(a.n) * n_used * J, cluster_pinned::kCpThreads);
         cluster_pinned::vtx_k_cp_pin<<<g, cluster_pinned::kCpThreads, 0, st>>>(a, pins, n_used, P<uint32_t>(ctx->cl_used_rows), K, n_rows,
                                                                              P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr));
         CK(cudaGetLastError());
@@ -1811,7 +1914,7 @@ static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uin
 
     // the EM: every active restart in the same launches; the host reads the restarts' flags and scores once per iteration
     if (n_used) {
-        const unsigned igrid = std::max(1u, std::min(blocks_for(uint64_t(R) * n_used * K, kClThreads), unsigned(ctx->n_sm) * 16));
+        const unsigned igrid = grid_for(ctx, uint64_t(R) * n_used * K, kClThreads);
         vtx_k_cl_init<<<igrid, kClThreads, 0, st>>>(params->seed, R, K, n_used, P<uint32_t>(ctx->cl_used_rows), n_rows,
                                                      P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr));
         CK(cudaGetLastError());
@@ -1829,7 +1932,7 @@ static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uin
     for (uint32_t it = 1; act.n; ++it) {
         CK(cudaMemsetAsync(ctx->cl_flags.p, 0, flag_bytes, st));
         if (n_cols) {
-            const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(act.n) * n_cols * 32, kClThreads), unsigned(ctx->n_sm) * 16));
+            const unsigned g = grid_for(ctx, uint64_t(act.n) * n_cols * 32, kClThreads);
             vtx_k_cl_estep<<<g, kClThreads, 0, st>>>(act, ce, n_cols, n_rows, K, P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr),
                                                      P<uint32_t>(ctx->cl_w), d_changed, d_score);
             CK(cudaGetLastError());
@@ -1846,7 +1949,7 @@ static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uin
         }
         act = next;
         if (act.n && n_used) {
-            const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(act.n) * n_used * 32, kClThreads), unsigned(ctx->n_sm) * 16));
+            const unsigned g = grid_for(ctx, uint64_t(act.n) * n_used * 32, kClThreads);
             vtx_k_cl_mstep<<<g, kClThreads, 0, st>>>(act, n_used, P<uint32_t>(ctx->cl_used_rows), P<uint32_t>(ctx->cl_row_start),
                                                      P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a),
                                                      P<uint32_t>(ctx->cl_w), n_cols, n_rows, K, P<int32_t>(ctx->cl_la), P<int32_t>(ctx->cl_lr));
@@ -1872,31 +1975,22 @@ static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uin
 
     // the final M-step over every row, then the scoring
     if (n_rows) {
-        const unsigned g = std::max(1u, std::min(blocks_for(n_rows * 32, kClThreads), unsigned(ctx->n_sm) * 16));
+        const unsigned g = grid_for(ctx, n_rows * 32, kClThreads);
         vtx_k_cl_final<<<g, kClThreads, 0, st>>>(perm, n_rows, P<uint32_t>(ctx->cl_row_start), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
                                                  P<uint32_t>(ctx->cl_a), P<uint32_t>(ctx->cl_w) + size_t(best) * n_cols * K, K,
                                                  P<int64_t>(ctx->cl_A), P<int64_t>(ctx->cl_T));
         CK(cudaGetLastError());
     }
     if (n_cols) {
-        const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_cols) * 32, kClThreads), unsigned(ctx->n_sm) * 8));
+        const unsigned g = grid_for(ctx, uint64_t(n_cols) * 32, kClThreads, 8);
         const int64_t* A = P<int64_t>(ctx->cl_A);
         const int64_t* T = P<int64_t>(ctx->cl_T);
         int64_t* ll = P<int64_t>(ctx->cl_ll);
         uint64_t* cnt = P<uint64_t>(ctx->cl_cnt);
-        using cluster_pinned::vtx_k_cl_score_pinned;
-        if (J) {
-            if (H <= 32) vtx_k_cl_score_pinned<1><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
-            else if (H <= 64) vtx_k_cl_score_pinned<2><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
-            else if (H <= 160) vtx_k_cl_score_pinned<5><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
-            else if (H <= 288) vtx_k_cl_score_pinned<9><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
-            else vtx_k_cl_score_pinned<17><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
-        }
-        else if (H <= 32) vtx_k_cl_score<1><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
-        else if (H <= 64) vtx_k_cl_score<2><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
-        else if (H <= 160) vtx_k_cl_score<5><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
-        else if (H <= 288) vtx_k_cl_score<9><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
-        else vtx_k_cl_score<17><<<g, kClThreads, 0, st>>>(ce, n_cols, K, A, T, ll, cnt);
+        // with J = 0 (vtx_cluster_cells) every lane takes theta(A, T)
+        by_kh(H, [&](auto kh) {
+            cluster_pinned::vtx_k_cl_score_pinned<decltype(kh)::value><<<g, kClThreads, 0, st>>>(ce, n_cols, K, pins, A, T, ll, cnt);
+        });
         CK(cudaGetLastError());
     }
     ctx->h_cl_ll.resize(size_t(n_cols) * H);
@@ -1924,34 +2018,30 @@ static int cluster_cells_run(vtx_ctx* ctx, const char* fn, uint64_t n, const uin
 int vtx_cluster_cells(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
                       const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const vtx_cluster_params* params, vtx_clusters* out)
 {
-    using namespace clusters;
     if (!ctx || !params || !out) return VTX_E_INVALID;
     *out = vtx_clusters{};
-    if (!ctx->finished || ctx->gather_pending)
-        return set_err(ctx, VTX_E_STATE, "vtx_cluster_cells: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const char* fn = "vtx_cluster_cells";
+    if (int rc = check_finished(ctx, fn)) return rc;
     const uint32_t K = params->k, R = params->restarts;
-    if (K < kMinK || K > kMaxK) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: k = %u; 2 to 32 clusters are supported", K);
-    if (R < 1 || R > kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_cells: %u restarts; 1 to 64 are supported", R);
-    return cluster_cells_run(ctx, "vtx_cluster_cells", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, params, PinSpec{}, out);
+    if (int rc = check_k(ctx, fn, K)) return rc;
+    if (R < 1 || R > clusters::kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "%s: %u restarts; 1 to 64 are supported", fn, R);
+    return cluster_cells_run(ctx, fn, n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, params, PinSpec{}, out);
 }
 
 int vtx_cluster_cells_pinned(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint32_t* col, const uint32_t* ref_cnt,
                              const uint32_t* alt_cnt, uint64_t n_rows, uint32_t n_cols, const uint8_t* dosage,
                              const vtx_cluster_pinned_params* params, vtx_clusters* out)
 {
-    using namespace clusters;
     if (!ctx || !params || !out) return VTX_E_INVALID;
     *out = vtx_clusters{};
     const char* fn = "vtx_cluster_cells_pinned";
-    if (!ctx->finished || ctx->gather_pending)
-        return set_err(ctx, VTX_E_STATE, "%s: submits are unfinished (call vtx_finish / vtx_finish_device first)", fn);
+    if (int rc = check_finished(ctx, fn)) return rc;
     const uint32_t K = params->k, R = params->restarts, J = params->n_pinned;
-    if (K < kMinK || K > kMaxK) return set_err(ctx, VTX_E_INVALID, "%s: k = %u; 2 to 32 clusters are supported", fn, K);
-    if (R < 1 || R > kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "%s: %u restarts; 1 to 64 are supported", fn, R);
+    if (int rc = check_k(ctx, fn, K)) return rc;
+    if (R < 1 || R > clusters::kMaxRestarts) return set_err(ctx, VTX_E_INVALID, "%s: %u restarts; 1 to 64 are supported", fn, R);
     if (J < 1 || J >= K) return set_err(ctx, VTX_E_INVALID, "%s: %u pinned samples; 1 to k - 1 = %u are supported", fn, J, K - 1);
     if (!dosage) return set_err(ctx, VTX_E_INVALID, "%s: dosage is NULL", fn);
-    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
-        return set_err(ctx, VTX_E_INVALID, "%s: error rate %g outside [1e-6, 0.25]", fn, params->error_rate);
+    if (int rc = check_error_rate(ctx, fn, params->error_rate)) return rc;
     if (params->rho_permille < 0 || params->rho_permille > ambient::kMaxPermille)
         return set_err(ctx, VTX_E_INVALID, "%s: rho_permille %d; 0 to 500", fn, params->rho_permille);
     const vtx_cluster_params cp{ K, R, params->seed };
@@ -1967,14 +2057,14 @@ int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     using namespace ambient;
     if (!ctx || !params || !out) return VTX_E_INVALID;
     *out = vtx_ambient{};
-    if (!ctx->finished || ctx->gather_pending)
-        return set_err(ctx, VTX_E_STATE, "vtx_donors_ambient: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const char* fn = "vtx_donors_ambient";
+    int rc = check_finished(ctx, fn);
+    if (rc) return rc;
     const uint32_t D = params->n_donors;
     const int32_t given = params->rho_permille;
     if (D < donors::kMinDonors || D > donors::kMaxDonors)
         return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: %u donors; 2 to 32 are supported", D);
-    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
-        return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: error rate %g outside [1e-6, 0.25]", params->error_rate);
+    if ((rc = check_error_rate(ctx, fn, params->error_rate))) return rc;
     if (given < -1 || given > kMaxPermille)
         return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: rho_permille %d; -1 (estimate) or 0 to 500", given);
     if (n && (!row || !col || !ref_cnt || !alt_cnt)) return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: an entry array is NULL");
@@ -1989,31 +2079,20 @@ int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     constexpr double kSlack = 1.125;
     const double need = (double(n) * 28 + double(n_rows) * 21 + double(n_cols) * (8 + 24 + 8.0 * H)) * kSlack;
     double avail = 0;
-    {
-        CK(cudaSetDevice(ctx->device));
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        size_t held = 0;
-        for (DBuf* b : { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_cell_count, &ctx->cl_cell_start,
-                         &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_ll, &ctx->cl_cnt, &ctx->am_sums, &ctx->am_tix,
-                         &ctx->am_touched, &ctx->am_dos, &ctx->am_tab, &ctx->am_grid })
-            held += b->cap;
-        avail = double(free_b) + double(held);
-        if (need > avail)
-            return set_err(ctx, VTX_E_NOMEM, "vtx_donors_ambient needs %.0f MB of device memory, %.0f MB are free", need * 1e-6, avail * 1e-6);
-    }
-    const size_t cells = size_t(n_rows) * D;
-    for (size_t i = 0; i < cells; ++i)
-        if (dosage[i] > 2 && dosage[i] != donors::kMissing)
-            return set_err(ctx, VTX_E_INVALID, "vtx_donors_ambient: dosage %u at row %zu, donor %zu (0, 1, 2 or VTX_GT_MISSING)",
-                           unsigned(dosage[i]), i / D, i % D);
+    rc = check_free(ctx, fn, need, { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_cell_count,
+                                     &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_ll, &ctx->cl_cnt,
+                                     &ctx->am_sums, &ctx->am_tix, &ctx->am_touched, &ctx->am_dos, &ctx->am_tab, &ctx->am_grid }, &avail);
+    if (rc) return rc;
     std::vector<uint8_t> usable(size_t(n_rows) + 1, 0);
     uint64_t rows_usable = 0;
-    for (uint64_t v = 0; v < n_rows; ++v) rows_usable += usable[v] = donors::row_usable(dosage + size_t(v) * D, D) ? 1 : 0;
+    for (uint64_t v = 0; v < n_rows; ++v) {
+        if ((rc = check_dosage_row(ctx, fn, dosage + size_t(v) * D, D, v, "donor"))) return rc;
+        rows_usable += usable[v] = donors::row_usable(dosage + size_t(v) * D, D) ? 1 : 0;
+    }
     // validate the entries in one pass; a usable row with an entry of r + a > 0 is "touched" and gets the next table index
     std::vector<uint32_t> tix(size_t(n_rows) + 1, 0), touched;
-    int rc = validate_entries(ctx, "vtx_donors_ambient", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxRowDepth,
-                              "its pool fraction would not be exact", [&](uint32_t v, uint64_t, uint64_t, uint64_t depth) {
+    rc = validate_entries(ctx, fn, n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxRowDepth,
+                          "its pool fraction would not be exact", [&](uint32_t v, uint64_t, uint64_t, uint64_t depth) {
         if (depth && usable[v]) { tix[v] = uint32_t(touched.size()); touched.push_back(v); }
     });
     if (rc) return rc;
@@ -2023,61 +2102,31 @@ int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     // the rest of the memory holds the tables of as many m as fit, at least one
     const double fixed = need + double(n_t) * (D + 4) * kSlack, per_m = double(n_t) * 40 * kSlack;
     if (fixed + per_m > avail)
-        return set_err(ctx, VTX_E_NOMEM, "vtx_donors_ambient needs %.0f MB of device memory, %.0f MB are free", (fixed + per_m) * 1e-6, avail * 1e-6);
+        return set_err(ctx, VTX_E_NOMEM, "%s needs %.0f MB of device memory, %.0f MB are free", fn, (fixed + per_m) * 1e-6, avail * 1e-6);
     uint32_t batch = kMaxBatch;
     if (per_m > 0) batch = uint32_t(std::min(double(kMaxBatch), std::floor((avail - fixed) / per_m)));
     if (params->grid_batch) batch = std::min(batch, params->grid_batch);
 
     cudaStream_t st = ctx->stream;
-    const size_t nb = size_t(n) * 4 + 4;
-    ENS(ctx->cl_row, nb); ENS(ctx->cl_col, nb); ENS(ctx->cl_r, nb); ENS(ctx->cl_a, nb);
-    ENS(ctx->cl_c_row, nb); ENS(ctx->cl_c_r, nb); ENS(ctx->cl_c_a, nb);
     ENS(ctx->cl_used, usable.size());
     ENS(ctx->am_tix, tix.size() * 4);
     ENS(ctx->am_touched, size_t(n_t) * 4 + 4);
     ENS(ctx->am_dos, dos.size());
-    ENS(ctx->am_sums, size_t(n_rows) * 16 + 16);
-    ENS(ctx->cl_cell_count, (size_t(n_cols) + 1) * 4);
-    ENS(ctx->cl_cell_start, (size_t(n_cols) + 1) * 4);
     ENS(ctx->cl_ll, size_t(n_cols) * H * 8 + 8); ENS(ctx->cl_cnt, size_t(n_cols) * 24 + 8);
     ENS(ctx->am_tab, size_t(batch) * n_t * 40 + 8);
     ENS(ctx->am_grid, size_t(kMaxBatch) * 4 * 8);
-    if (n) {
-        CK(cudaMemcpyAsync(ctx->cl_row.p, row, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_r.p, ref_cnt, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_a.p, alt_cnt, n * 4, cudaMemcpyHostToDevice, st));
-    }
     CK(cudaMemcpyAsync(ctx->cl_used.p, usable.data(), usable.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->am_tix.p, tix.data(), tix.size() * 4, cudaMemcpyHostToDevice, st));
     if (n_t) {
         CK(cudaMemcpyAsync(ctx->am_touched.p, touched.data(), size_t(n_t) * 4, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(ctx->am_dos.p, dos.data(), size_t(n_t) * D, cudaMemcpyHostToDevice, st));
     }
-    unsigned long long* d_A = P<unsigned long long>(ctx->am_sums);
-    unsigned long long* d_T = d_A + n_rows;
-    CK(cudaMemsetAsync(ctx->am_sums.p, 0, size_t(n_rows) * 16, st));
 
-    // A_v, T_v and the by-cell index of the kept entries (§5g's kernels with used = the usable rows)
-    const uint32_t nn = uint32_t(n);
-    const unsigned egrid = std::max(1u, std::min(blocks_for(n, kAmThreads), unsigned(ctx->n_sm) * 16));
-    if (n) {
-        vtx_k_am_rowsum<<<egrid, kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a), d_A, d_T);
-        CK(cudaGetLastError());
-    }
-    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
-    clusters::vtx_k_cl_count<<<egrid, kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
-                                                  P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_count));
-    CK(cudaGetLastError());
-    rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->cl_cell_count), n_cols, P<uint32_t>(ctx->cl_cell_start), nullptr);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
-    clusters::vtx_k_cl_scatter<<<egrid, kAmThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
-                                                    P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_start),
-                                                    P<uint32_t>(ctx->cl_cell_count), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r),
-                                                    P<uint32_t>(ctx->cl_c_a));
-    CK(cudaGetLastError());
-    const clusters::CellEntries ce{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
+    // the by-cell index of the kept entries (§5g's kernels with used = the usable rows), then A_v, T_v
+    clusters::CellEntries ce;
+    if ((rc = cell_entries(ctx, n, row, col, ref_cnt, alt_cnt, n_cols, &ce))) return rc;
+    const unsigned long long *d_A, *d_T;
+    if ((rc = pool_row_sums(ctx, n, n_rows, &d_A, &d_T))) return rc;
 
     // J(m) and the calls of every m in `ms`, `batch` m per pass; with `final` (one m), also the cells' log-likelihoods
     const Fractions fr = fractions(params->error_rate);
@@ -2091,22 +2140,20 @@ int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
             for (uint32_t b = 0; b < bt.n; ++b) bt.m[b] = ms[o + b];
             CK(cudaMemsetAsync(ctx->am_grid.p, 0, h_grid.size() * 8, st));
             if (n_t) {
-                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_t, kAmThreads), unsigned(ctx->n_sm) * 16));
+                const unsigned g = grid_for(ctx, uint64_t(bt.n) * n_t, kAmThreads);
                 vtx_k_am_tables<<<g, kAmThreads, 0, st>>>(bt, fr, n_t, P<uint32_t>(ctx->am_touched), d_A, d_T, P<int32_t>(ctx->am_tab));
                 CK(cudaGetLastError());
             }
             if (n_cols) {
-                const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(bt.n) * n_cols * 32, kAmThreads), unsigned(ctx->n_sm) * 16));
+                const unsigned g = grid_for(ctx, uint64_t(bt.n) * n_cols * 32, kAmThreads);
                 const uint32_t* tx = P<uint32_t>(ctx->am_tix);
                 const uint8_t* dd = P<uint8_t>(ctx->am_dos);
                 const int32_t* tb = P<int32_t>(ctx->am_tab);
                 int64_t* ll = final ? P<int64_t>(ctx->cl_ll) : nullptr;
                 uint64_t* cnt = final ? P<uint64_t>(ctx->cl_cnt) : nullptr;
-                if (H <= 32) vtx_k_am_score<1><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
-                else if (H <= 64) vtx_k_am_score<2><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
-                else if (H <= 160) vtx_k_am_score<5><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
-                else if (H <= 288) vtx_k_am_score<9><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
-                else vtx_k_am_score<17><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
+                by_kh(H, [&](auto kh) {
+                    vtx_k_am_score<decltype(kh)::value><<<g, kAmThreads, 0, st>>>(bt, ce, n_cols, D, tx, dd, tb, n_t, d_J, d_calls, ll, cnt);
+                });
                 CK(cudaGetLastError());
             }
             CK(cudaMemcpyAsync(h_grid.data(), ctx->am_grid.p, h_grid.size() * 8, cudaMemcpyDeviceToHost, st));
@@ -2131,15 +2178,7 @@ int vtx_donors_ambient(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     rc = evaluate({ uint16_t(chosen) }, true, &obj_f, &calls_f);
     if (rc) return rc;
     if (given >= 0) { ms.assign(1, uint16_t(chosen)); obj = obj_f; calls = calls_f; }
-    std::vector<size_t> order(ms.size());
-    for (size_t i = 0; i < order.size(); ++i) order[i] = i;
-    std::sort(order.begin(), order.end(), [&](size_t x, size_t y) { return ms[x] < ms[y]; });
-    ctx->h_am_m.resize(ms.size()); ctx->h_am_obj.resize(ms.size()); ctx->h_am_calls.resize(ms.size() * 3);
-    for (size_t i = 0; i < order.size(); ++i) {
-        ctx->h_am_m[i] = ms[order[i]];
-        ctx->h_am_obj[i] = obj[order[i]];
-        for (int k = 0; k < 3; ++k) ctx->h_am_calls[3 * i + k] = calls[3 * order[i] + k];
-    }
+    sort_grid(ms, obj, &calls, ctx->h_am_m, ctx->h_am_obj, &ctx->h_am_calls);
 
     ctx->h_am_ll.resize(size_t(n_cols) * H);
     ctx->h_am_cnt.resize(size_t(n_cols) * 3);
@@ -2170,16 +2209,15 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
     using namespace cluster_gt;
     if (!ctx || !params || !out) return VTX_E_INVALID;
     *out = vtx_cluster_gt{};
-    if (!ctx->finished || ctx->gather_pending)
-        return set_err(ctx, VTX_E_STATE, "vtx_cluster_genotypes: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const char* fn = "vtx_cluster_genotypes";
+    int rc = check_finished(ctx, fn);
+    if (rc) return rc;
     const uint32_t K = params->k, S = params->n_samples;
     const int32_t given = params->rho_permille;
-    if (K < clusters::kMinK || K > clusters::kMaxK)
-        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: k = %u; 2 to 32 clusters are supported", K);
+    if ((rc = check_k(ctx, fn, K))) return rc;
     if (S > kMaxSamples) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: %u samples; 0 to 1024 are supported", S);
     if (S && !dosage) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: dosage is NULL");
-    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
-        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: error rate %g outside [1e-6, 0.25]", params->error_rate);
+    if ((rc = check_error_rate(ctx, fn, params->error_rate))) return rc;
     if (given < -1 || given > ambient::kMaxPermille)
         return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: rho_permille %d; -1 (estimate) or 0 to 500", given);
     if (n_rows && (!alt_w || !depth_w || !row_used || !row_alt || !row_depth))
@@ -2192,28 +2230,13 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
     std::vector<uint32_t> touched, fit, cmp;
     uint64_t total = 0, rows_compared = 0;
     for (uint64_t v = 0; v < n_rows; ++v) {
-        bool reached = false;
-        for (uint32_t k = 0; k < K; ++k) {
-            const int64_t a = alt_w[v * K + k], t = depth_w[v * K + k];
-            if (a < 0 || a > t || t > kMaxDepthW)
-                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: row %llu, cluster %u: alt_w %lld, depth_w %lld (0 <= alt_w <= depth_w <= 2^51)",
-                               (unsigned long long)v, k, (long long)a, (long long)t);
-            total += uint64_t(t);
-            if (total > kMaxTotalDepthW)
-                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: depth_w sums to more than 2^51 over the rows; the fit's int64 sums would not be exact");
-            reached = reached || t > 0;
-        }
+        if ((rc = check_sums_row(ctx, fn, alt_w + v * K, depth_w + v * K, K, v, &total))) return rc;
+        const bool reached = std::any_of(depth_w + v * K, depth_w + (v + 1) * K, [](int64_t t) { return t > 0; });
         if (row_alt[v] > row_depth[v] || row_depth[v] > ambient::kMaxRowDepth)
             return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: row %llu: row_alt %llu, row_depth %llu (row_alt <= row_depth < 2^53 - 2)",
                            (unsigned long long)v, (unsigned long long)row_alt[v], (unsigned long long)row_depth[v]);
-        bool all = S > 0;
-        for (uint32_t s = 0; s < S; ++s) {
-            const uint8_t g = dosage[v * S + s];
-            if (g > 2 && g != kMissing)
-                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_genotypes: dosage %u at row %llu, sample %u (0, 1, 2 or VTX_GT_MISSING)",
-                               unsigned(g), (unsigned long long)v, s);
-            all = all && g != kMissing;
-        }
+        if ((rc = check_dosage_row(ctx, fn, dosage + v * S, S, v, "sample"))) return rc;
+        const bool all = S > 0 && std::none_of(dosage + v * S, dosage + (v + 1) * S, [](uint8_t g) { return g == kMissing; });
         rows_compared += all;
         if (!reached) continue;
         if (row_used[v]) fit.push_back(uint32_t(touched.size()));
@@ -2221,18 +2244,11 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
         touched.push_back(uint32_t(v));
     }
     const uint32_t n_t = uint32_t(touched.size()), n_fit = uint32_t(fit.size()), n_cmp = uint32_t(cmp.size());
-    {   // every buffer is allocated with 1/8 to spare (ensure)
-        const double need = (double(n_t) * (53.0 * K + 16) + double(n_fit) * 4 + double(n_cmp) * (4.0 + S) + 16.0 * K * (S + 1) + 4096) * 1.125;
-        CK(cudaSetDevice(ctx->device));
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        size_t held = 0;
-        for (DBuf* b : { &ctx->cg_AT, &ctx->cg_rows, &ctx->cg_fit, &ctx->cg_ll, &ctx->cg_gt, &ctx->cg_pl, &ctx->cg_cmp, &ctx->cg_dos, &ctx->cg_acc })
-            held += b->cap;
-        if (need > double(free_b) + double(held))
-            return set_err(ctx, VTX_E_NOMEM, "vtx_cluster_genotypes needs %.0f MB of device memory, %.0f MB are free", need * 1e-6,
-                           (double(free_b) + double(held)) * 1e-6);
-    }
+    // every buffer is allocated with 1/8 to spare (ensure)
+    const double need = (double(n_t) * (53.0 * K + 16) + double(n_fit) * 4 + double(n_cmp) * (4.0 + S) + 16.0 * K * (S + 1) + 4096) * 1.125;
+    rc = check_free(ctx, fn, need, { &ctx->cg_AT, &ctx->cg_rows, &ctx->cg_fit, &ctx->cg_ll, &ctx->cg_gt, &ctx->cg_pl, &ctx->cg_cmp,
+                                     &ctx->cg_dos, &ctx->cg_acc });
+    if (rc) return rc;
     // the touched rows' inputs, compacted: A, T [touched][K], then A_v, T_v [touched]; the compared rows' dosages
     std::vector<int64_t> at(size_t(n_t) * K * 2);
     std::vector<uint64_t> rows(size_t(n_t) * 2);
@@ -2273,7 +2289,7 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
     std::vector<uint16_t> ms;
     std::vector<int64_t> obj;
     uint32_t chosen = 0;
-    const int rc = cg_fit_device(ctx, fr, K, given, n_t, n_fit, P<uint32_t>(ctx->cg_fit), d_rowA, d_rowT, d_A, d_T, ms, obj, &chosen);
+    rc = cg_fit_device(ctx, fr, K, given, n_t, n_fit, P<uint32_t>(ctx->cg_fit), d_rowA, d_rowT, d_A, d_T, ms, obj, &chosen);
     if (rc) return rc;
     unsigned long long* d_M = d_J + ambient::kMaxBatch;
     const size_t n_acc = 2 * size_t(K) * S + 2 * K;                   // M, discordant [K][S], then rows, called [K]
@@ -2300,11 +2316,7 @@ int vtx_cluster_genotypes(vtx_ctx* ctx, uint64_t n_rows, const int64_t* alt_w, c
     CK(cudaMemcpyAsync(ctx->h_cg_acc.data(), d_M, n_acc * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
 
-    std::vector<size_t> order(ms.size());
-    for (size_t i = 0; i < order.size(); ++i) order[i] = i;
-    std::sort(order.begin(), order.end(), [&](size_t x, size_t y) { return ms[x] < ms[y]; });
-    ctx->h_cg_m.resize(ms.size()); ctx->h_cg_obj.resize(ms.size());
-    for (size_t i = 0; i < order.size(); ++i) { ctx->h_cg_m[i] = ms[order[i]]; ctx->h_cg_obj[i] = obj[order[i]]; }
+    sort_grid(ms, obj, nullptr, ctx->h_cg_m, ctx->h_cg_obj, nullptr);
     ctx->h_cg_touched.assign(touched.begin(), touched.end());
     ctx->h_cg_M.resize(size_t(K) * S);
     for (size_t i = 0; i < ctx->h_cg_M.size(); ++i) ctx->h_cg_M[i] = int64_t(ctx->h_cg_acc[i]);
@@ -2325,13 +2337,12 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     using namespace cluster_refine;
     if (!ctx || !params || !out) return VTX_E_INVALID;
     *out = vtx_cluster_calls{};
-    if (!ctx->finished || ctx->gather_pending)
-        return set_err(ctx, VTX_E_STATE, "vtx_cluster_refine: submits are unfinished (call vtx_finish / vtx_finish_device first)");
+    const char* fn = "vtx_cluster_refine";
+    int rc = check_finished(ctx, fn);
+    if (rc) return rc;
     const uint32_t K = params->k, max_rounds = params->max_rounds;
-    if (K < clusters::kMinK || K > clusters::kMaxK)
-        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: k = %u; 2 to 32 clusters are supported", K);
-    if (!(params->error_rate >= 1e-6 && params->error_rate <= 0.25))
-        return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: error rate %g outside [1e-6, 0.25]", params->error_rate);
+    if ((rc = check_k(ctx, fn, K))) return rc;
+    if ((rc = check_error_rate(ctx, fn, params->error_rate))) return rc;
     if (max_rounds > kMaxRounds) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: max_rounds %u; 0 to 32 are supported", max_rounds);
     if (n && (!row || !col || !ref_cnt || !alt_cnt)) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: an entry array is NULL");
     if (n_rows && (!alt_w || !depth_w || !row_used)) return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: a row array is NULL");
@@ -2342,38 +2353,21 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     // device memory, before any host table of n_rows entries: the entries (16 B) and their by-cell copy (12 B); per row the flags,
     // scans, row sums and the round's sums, and at most every row touched and scored (the compacted fit, codes and tables); per
     // cell the weights, labels, log-likelihoods and counts.  Every buffer is allocated with 1/8 to spare (ensure).
-    {
-        const double need = (double(n) * 28 + double(n_rows) * (70.0 * K + 150) + double(n_cols) * (4.0 * K + 8.0 * H + 40) + 4096) * 1.125;
-        CK(cudaSetDevice(ctx->device));
-        size_t free_b = 0, total_b = 0;
-        CK(cudaMemGetInfo(&free_b, &total_b));
-        size_t held = 0;
-        for (DBuf* b : { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_row_start, &ctx->cl_cell_count,
-                         &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_w, &ctx->cl_A, &ctx->cl_T, &ctx->cl_ll,
-                         &ctx->cl_cnt, &ctx->am_sums, &ctx->cg_AT, &ctx->cg_rows, &ctx->cg_fit, &ctx->cg_ll, &ctx->cg_gt, &ctx->cg_pl,
-                         &ctx->cg_acc, &ctx->cr_rowflags, &ctx->cr_code, &ctx->cr_sflag, &ctx->cr_scode, &ctx->cr_tab, &ctx->cr_label,
-                         &ctx->cr_scal })
-            held += b->cap;
-        if (need > double(free_b) + double(held))
-            return set_err(ctx, VTX_E_NOMEM, "vtx_cluster_refine needs %.0f MB of device memory, %.0f MB are free", need * 1e-6,
-                           (double(free_b) + double(held)) * 1e-6);
-    }
+    const double need = (double(n) * 28 + double(n_rows) * (70.0 * K + 150) + double(n_cols) * (4.0 * K + 8.0 * H + 40) + 4096) * 1.125;
+    rc = check_free(ctx, fn, need, { &ctx->cl_row, &ctx->cl_col, &ctx->cl_r, &ctx->cl_a, &ctx->cl_used, &ctx->cl_row_start,
+                                     &ctx->cl_cell_count, &ctx->cl_cell_start, &ctx->cl_c_row, &ctx->cl_c_r, &ctx->cl_c_a, &ctx->cl_w,
+                                     &ctx->cl_A, &ctx->cl_T, &ctx->cl_ll, &ctx->cl_cnt, &ctx->am_sums, &ctx->cg_AT, &ctx->cg_rows,
+                                     &ctx->cg_fit, &ctx->cg_ll, &ctx->cg_gt, &ctx->cg_pl, &ctx->cg_acc, &ctx->cr_rowflags, &ctx->cr_code,
+                                     &ctx->cr_sflag, &ctx->cr_scode, &ctx->cr_tab, &ctx->cr_label, &ctx->cr_scal });
+    if (rc) return rc;
     // validate once: §5i's bounds on the sums, then the entries, whose total bounds every later round's hard sums
     uint64_t total = 0;
     for (uint64_t v = 0; v < n_rows; ++v)
-        for (uint32_t k = 0; k < K; ++k) {
-            const int64_t a = alt_w[v * K + k], t = depth_w[v * K + k];
-            if (a < 0 || a > t || t > cluster_gt::kMaxDepthW)
-                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: row %llu, cluster %u: alt_w %lld, depth_w %lld (0 <= alt_w <= depth_w <= 2^51)",
-                               (unsigned long long)v, k, (long long)a, (long long)t);
-            total += uint64_t(t);
-            if (total > cluster_gt::kMaxTotalDepthW)
-                return set_err(ctx, VTX_E_INVALID, "vtx_cluster_refine: depth_w sums to more than 2^51 over the rows; the fit's int64 sums would not be exact");
-        }
+        if ((rc = check_sums_row(ctx, fn, alt_w + v * K, depth_w + v * K, K, v, &total))) return rc;
     std::vector<uint32_t> row_start(size_t(n_rows) + 1, 0);
     uint64_t molecules = 0;
-    int rc = validate_entries(ctx, "vtx_cluster_refine", n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxTotalMolecules,
-                              "its hard sums would not be exact", [&](uint32_t v, uint64_t i0, uint64_t i1, uint64_t m) {
+    rc = validate_entries(ctx, fn, n, row, col, ref_cnt, alt_cnt, n_rows, n_cols, kMaxTotalMolecules,
+                          "its hard sums would not be exact", [&](uint32_t v, uint64_t i0, uint64_t i1, uint64_t m) {
         row_start[size_t(v) + 1] = uint32_t(i1 - i0);
         molecules += m;
     });
@@ -2383,59 +2377,29 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     for (uint64_t v = 0; v < n_rows; ++v) row_start[v + 1] += row_start[v];
 
     cudaStream_t st = ctx->stream;
-    const size_t nb = size_t(n) * 4 + 4;
-    ENS(ctx->cl_row, nb); ENS(ctx->cl_col, nb); ENS(ctx->cl_r, nb); ENS(ctx->cl_a, nb);
-    ENS(ctx->cl_c_row, nb); ENS(ctx->cl_c_r, nb); ENS(ctx->cl_c_a, nb);
     ENS(ctx->cl_used, size_t(n_rows) + 1);
     ENS(ctx->cl_row_start, row_start.size() * 4);
-    ENS(ctx->cl_cell_count, (size_t(n_cols) + 1) * 4);
-    ENS(ctx->cl_cell_start, (size_t(n_cols) + 1) * 4);
     ENS(ctx->cl_w, size_t(n_cols) * K * 4 + 4);
     ENS(ctx->cl_A, size_t(n_rows) * K * 8 + 8); ENS(ctx->cl_T, size_t(n_rows) * K * 8 + 8);
     ENS(ctx->cl_ll, size_t(n_cols) * H * 8 + 8); ENS(ctx->cl_cnt, size_t(n_cols) * 24 + 8);
-    ENS(ctx->am_sums, size_t(n_rows) * 16 + 16);
     ENS(ctx->cg_acc, size_t(ambient::kMaxBatch) * 8);
     const size_t rf = size_t(n_rows) + 1;                   // tflag, tpos, fflag, fpos, sidx: n_rows + 1 each
     ENS(ctx->cr_rowflags, rf * 5 * 4);
     ENS(ctx->cr_label, size_t(n_cols) * 8 + 8);
     ENS(ctx->cr_scal, 4 * 8);
-    if (n) {
-        CK(cudaMemcpyAsync(ctx->cl_row.p, row, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_r.p, ref_cnt, n * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->cl_a.p, alt_cnt, n * 4, cudaMemcpyHostToDevice, st));
-    }
     CK(cudaMemcpyAsync(ctx->cl_row_start.p, row_start.data(), row_start.size() * 4, cudaMemcpyHostToDevice, st));
     if (n_rows) {
         CK(cudaMemcpyAsync(ctx->cl_A.p, alt_w, size_t(n_rows) * K * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(ctx->cl_T.p, depth_w, size_t(n_rows) * K * 8, cudaMemcpyHostToDevice, st));
     }
-    unsigned long long* d_rowA = P<unsigned long long>(ctx->am_sums);
-    unsigned long long* d_rowT = d_rowA + n_rows;
-    CK(cudaMemsetAsync(ctx->am_sums.p, 0, size_t(n_rows) * 16, st));
 
-    // A_v, T_v and the by-cell index of every entry with r + a > 0 (§5g's kernels with every row kept); then `used` becomes row_used
-    const uint32_t nn = uint32_t(n);
-    const unsigned egrid = std::max(1u, std::min(blocks_for(n, kCrThreads), unsigned(ctx->n_sm) * 16));
-    if (n) {
-        ambient::vtx_k_am_rowsum<<<egrid, kCrThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a), d_rowA, d_rowT);
-        CK(cudaGetLastError());
-    }
+    // the by-cell index of every entry with r + a > 0 (§5g's kernels with every row kept), then A_v, T_v; then `used` becomes row_used
     CK(cudaMemsetAsync(ctx->cl_used.p, 1, size_t(n_rows) + 1, st));
-    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
-    clusters::vtx_k_cl_count<<<egrid, kCrThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
-                                                           P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_count));
-    CK(cudaGetLastError());
-    rc = scan_u32(ctx, st, ctx->scan_sums, P<uint32_t>(ctx->cl_cell_count), n_cols, P<uint32_t>(ctx->cl_cell_start), nullptr);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(ctx->cl_cell_count.p, 0, (size_t(n_cols) + 1) * 4, st));
-    clusters::vtx_k_cl_scatter<<<egrid, kCrThreads, 0, st>>>(nn, P<uint32_t>(ctx->cl_row), P<uint32_t>(ctx->cl_col), P<uint32_t>(ctx->cl_r),
-                                                             P<uint32_t>(ctx->cl_a), P<uint8_t>(ctx->cl_used), P<uint32_t>(ctx->cl_cell_start),
-                                                             P<uint32_t>(ctx->cl_cell_count), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r),
-                                                             P<uint32_t>(ctx->cl_c_a));
-    CK(cudaGetLastError());
+    clusters::CellEntries ce;
+    if ((rc = cell_entries(ctx, n, row, col, ref_cnt, alt_cnt, n_cols, &ce))) return rc;
+    const unsigned long long *d_rowA, *d_rowT;
+    if ((rc = pool_row_sums(ctx, n, n_rows, &d_rowA, &d_rowT))) return rc;
     if (n_rows) CK(cudaMemcpyAsync(ctx->cl_used.p, row_used, n_rows, cudaMemcpyHostToDevice, st));
-    const clusters::CellEntries ce{ P<uint32_t>(ctx->cl_cell_start), P<uint32_t>(ctx->cl_c_row), P<uint32_t>(ctx->cl_c_r), P<uint32_t>(ctx->cl_c_a) };
     uint32_t* d_tflag = P<uint32_t>(ctx->cr_rowflags);
     uint32_t* d_tpos = d_tflag + rf;
     uint32_t* d_fflag = d_tpos + rf;
@@ -2447,7 +2411,7 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     CK(cudaMemsetAsync(d_prev, 0xFF, size_t(n_cols) * 4, st));              // round 0 compares with VTX_NO_LABEL
 
     const ambient::Fractions fr = ambient::fractions(params->error_rate);
-    const unsigned rgrid = std::max(1u, std::min(blocks_for(n_rows, kCrThreads), unsigned(ctx->n_sm) * 16));
+    const unsigned rgrid = grid_for(ctx, n_rows, kCrThreads);
     clusters::Perm ident{};
     for (uint32_t k = 0; k < K; ++k) ident.k[k] = uint8_t(k);
     ctx->h_cr_rounds.clear();
@@ -2455,7 +2419,7 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
     uint32_t n_t = 0;
     for (uint32_t r = 0;; ++r) {
         if (r > 0 && n_rows) {       // the previous round's labels' hard sums
-            const unsigned g = std::max(1u, std::min(blocks_for(n_rows * 32, clusters::kClThreads), unsigned(ctx->n_sm) * 16));
+            const unsigned g = grid_for(ctx, n_rows * 32, clusters::kClThreads);
             clusters::vtx_k_cl_final<<<g, clusters::kClThreads, 0, st>>>(ident, n_rows, P<uint32_t>(ctx->cl_row_start), P<uint32_t>(ctx->cl_col),
                                                                          P<uint32_t>(ctx->cl_r), P<uint32_t>(ctx->cl_a), P<uint32_t>(ctx->cl_w), K,
                                                                          P<int64_t>(ctx->cl_A), P<int64_t>(ctx->cl_T));
@@ -2500,7 +2464,7 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
         if (rc) return rc;
         uint32_t n_s = 0;
         if (n_t) {
-            const unsigned g = std::max(1u, std::min(blocks_for(n_t, kCrThreads), unsigned(ctx->n_sm) * 16));
+            const unsigned g = grid_for(ctx, n_t, kCrThreads);
             vtx_k_cr_codes<<<g, kCrThreads, 0, st>>>(n_t, K, P<uint8_t>(ctx->cg_gt), P<uint32_t>(ctx->cg_pl), P<uint8_t>(ctx->cr_code), d_sflag);
             CK(cudaGetLastError());
             rc = scan_u32(ctx, st, ctx->scan_sums, d_sflag, n_t, d_spos, nullptr);
@@ -2512,7 +2476,7 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
         ENS(ctx->cr_tab, size_t(n_s) * kEntries * 8 + 8);
         if (n_rows) CK(cudaMemsetAsync(d_sidx, 0xFF, size_t(n_rows) * 4, st));
         if (n_s) {
-            const unsigned g = std::max(1u, std::min(blocks_for(n_t, kCrThreads), unsigned(ctx->n_sm) * 16));
+            const unsigned g = grid_for(ctx, n_t, kCrThreads);
             vtx_k_cr_tables<<<g, kCrThreads, 0, st>>>(m, fr, n_t, K, d_trow, d_crow, P<uint8_t>(ctx->cr_code), d_sflag, d_spos, d_sidx,
                                                       P<uint8_t>(ctx->cr_scode), P<int32_t>(ctx->cr_tab));
             CK(cudaGetLastError());
@@ -2520,19 +2484,17 @@ int vtx_cluster_refine(vtx_ctx* ctx, uint64_t n, const uint32_t* row, const uint
         // the cells: scores, calls and labels; the next round's weights and the changed labels
         CK(cudaMemsetAsync(d_scal, 0, 4 * 8, st));
         if (n_cols) {
-            const unsigned g = std::max(1u, std::min(blocks_for(uint64_t(n_cols) * 32, kCrThreads), unsigned(ctx->n_sm) * 8));
+            const unsigned g = grid_for(ctx, uint64_t(n_cols) * 32, kCrThreads, 8);
             const uint32_t* sx = d_sidx;
             const uint8_t* sc = P<uint8_t>(ctx->cr_scode);
             const int32_t* tb = P<int32_t>(ctx->cr_tab);
             int64_t* ll = P<int64_t>(ctx->cl_ll);
             uint64_t* cnt = P<uint64_t>(ctx->cl_cnt);
-            if (H <= 32) vtx_k_cr_score<1><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
-            else if (H <= 64) vtx_k_cr_score<2><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
-            else if (H <= 160) vtx_k_cr_score<5><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
-            else if (H <= 288) vtx_k_cr_score<9><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
-            else vtx_k_cr_score<17><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
+            by_kh(H, [&](auto kh) {
+                vtx_k_cr_score<decltype(kh)::value><<<g, kCrThreads, 0, st>>>(ce, n_cols, K, sx, sc, tb, ll, cnt, d_label, d_scal);
+            });
             CK(cudaGetLastError());
-            const unsigned wg = std::max(1u, std::min(blocks_for(n_cols, kCrThreads), unsigned(ctx->n_sm) * 16));
+            const unsigned wg = grid_for(ctx, n_cols, kCrThreads);
             vtx_k_cr_weights<<<wg, kCrThreads, 0, st>>>(n_cols, K, d_label, d_prev, P<uint32_t>(ctx->cl_w), d_scal + 3);
             CK(cudaGetLastError());
         }

@@ -8,11 +8,13 @@
 // entries s = 2g at m, written over §5g's init and again after every M-step; where sample j has no dosage, cluster j is an
 // ordinary §5g cluster.  The final scoring forms the pinned theta_jv in row_log's expressions and feeds it to §5g's pair_logs;
 // every other (row, cluster) takes theta(A, T).  The same correctly rounded operations as §5g and §5h, so
-// tests/cluster_pinned_oracle.py reproduces the result bit for bit.
+// tests/cluster_pinned_oracle.py reproduces the result bit for bit.  With J = 0 (Pins{}) the scoring is §5g's, so
+// vtx_cluster_cells scores with vtx_k_cl_score_pinned too.
 //
 // Kernels (the rest is §5g's: vtx_k_cl_count / scan / scatter / init / estep / mstep / final, and §5h's vtx_k_am_rowsum):
 //   vtx_k_cp_pin             one thread per (active restart, used row, pinned sample): the pinned La / Lr where there is a dosage
-//   vtx_k_cl_score_pinned    vtx_k_cl_score with lane j < J forming the pinned theta where sample j has a dosage at the row
+//   vtx_k_cl_score_pinned    one warp per cell, lane l owning hypotheses l + 32j: the singlet / doublet log-likelihoods, with
+//                            lane j < J forming the pinned theta where sample j has a dosage at the row
 //
 // The per-item bodies are __host__ __device__ (plain C++ without nvcc): tests/cluster_pinned_shim.cpp runs them serially on the
 // CPU (tests/test_cluster_pinned_cpu.py).
@@ -81,23 +83,8 @@ VTX_CP_HD inline void cluster_theta(const Pins& p, uint32_t K, size_t v, uint32_
 inline void score_cell(const clusters::CellEntries& ce, uint32_t c, uint32_t K, const Pins& p, const int64_t* A, const int64_t* T,
                        int64_t* ll, uint64_t* cnt)
 {
-    const uint32_t H = donors::n_hyp(K);
-    for (uint32_t h = 0; h < H; ++h) ll[h] = 0;
-    cnt[0] = cnt[1] = cnt[2] = 0;
-    for (uint32_t i = ce.start[c]; i < ce.start[c + 1]; ++i) {
-        const size_t v = ce.row[i];
-        for (uint32_t h = 0; h < H; ++h) {
-            uint32_t d1, d2;
-            donors::hyp_donors(h, K, &d1, &d2);
-            double ti, oi, tj, oj;
-            cluster_theta(p, K, v, d1, A, T, &ti, &oi);
-            cluster_theta(p, K, v, d2, A, T, &tj, &oj);
-            int32_t la, lr;
-            clusters::pair_logs(ti, oi, tj, oj, &la, &lr);
-            ll[h] += int64_t(ce.r[i]) * lr + int64_t(ce.a[i]) * la;
-        }
-        cnt[0] += 1; cnt[1] += ce.r[i]; cnt[2] += ce.a[i];
-    }
+    clusters::score_cell_by(ce, c, K, [&](size_t v, uint32_t j, double* th, double* om) { cluster_theta(p, K, v, j, A, T, th, om); },
+                            ll, cnt);
 }
 
 #ifdef __CUDACC__
@@ -119,7 +106,8 @@ __global__ void __launch_bounds__(kCpThreads) vtx_k_cp_pin(clusters::Active act,
     }
 }
 
-// One warp per cell: vtx_k_cl_score, with lane j < K taking cluster_theta at the entry's row
+// One warp per cell.  Lane k < K forms its cluster's theta and 1 - theta at the entry's row (cluster_theta); lane l then takes
+// the two clusters of each of its hypotheses h = l + 32j (j < KH = ceil(H / 32)) by shuffle.
 template <int KH>
 __global__ void __launch_bounds__(kCpThreads) vtx_k_cl_score_pinned(clusters::CellEntries ce, uint32_t n_cols, uint32_t K, Pins p,
                                                                     const int64_t* __restrict__ A, const int64_t* __restrict__ T,

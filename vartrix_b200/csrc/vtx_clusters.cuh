@@ -19,7 +19,7 @@
 //   vtx_k_cl_estep     one warp per (cell, active restart): W, the restart's "changed" flag and score
 //   vtx_k_cl_mstep     one warp per (used row, active restart): the next La / Lr, no atomics
 //   vtx_k_cl_final     one warp per row (every row), the best restart: A, T in the canonical cluster order
-//   vtx_k_cl_score     one warp per cell, lane l owns hypotheses l + 32j: the singlet / doublet log-likelihoods
+// The singlet / doublet scoring is vtx_cluster_pinned.cuh's vtx_k_cl_score_pinned with no pinned sample (J = 0).
 //
 // The per-item bodies are __host__ __device__ (plain C++ without nvcc): tests/cluster_shim.cpp runs them serially on the CPU
 // (tests/test_clusters_cpu.py).  That build must not contract either (g++ does not on x86-64 without -mfma).
@@ -224,8 +224,10 @@ inline void mstep_row(const uint32_t* col, const uint32_t* r, const uint32_t* a,
         }
 }
 
-// final scoring of cell c from A, T [n_rows][K] (canonical order): ll[H], cnt[3] = variants, ref, alt
-inline void score_cell(const CellEntries& ce, uint32_t c, uint32_t K, const int64_t* A, const int64_t* T, int64_t* ll, uint64_t* cnt)
+// final scoring of cell c: ll[H], cnt[3] = variants, ref, alt; theta_of(v, k, &th, &om) gives canonical cluster k's theta and
+// 1 - theta at row v (vtx_cluster_pinned.cuh's score_cell passes its pinned theta)
+template <typename ThetaOf>
+inline void score_cell_by(const CellEntries& ce, uint32_t c, uint32_t K, ThetaOf theta_of, int64_t* ll, uint64_t* cnt)
 {
     const uint32_t H = donors::n_hyp(K);
     for (uint32_t h = 0; h < H; ++h) ll[h] = 0;
@@ -236,14 +238,20 @@ inline void score_cell(const CellEntries& ce, uint32_t c, uint32_t K, const int6
             uint32_t d1, d2;
             donors::hyp_donors(h, K, &d1, &d2);
             double ti, oi, tj, oj;
-            theta(A[v * K + d1], T[v * K + d1], &ti, &oi);
-            theta(A[v * K + d2], T[v * K + d2], &tj, &oj);
+            theta_of(v, d1, &ti, &oi);
+            theta_of(v, d2, &tj, &oj);
             int32_t la, lr;
             pair_logs(ti, oi, tj, oj, &la, &lr);
             ll[h] += int64_t(ce.r[i]) * lr + int64_t(ce.a[i]) * la;
         }
         cnt[0] += 1; cnt[1] += ce.r[i]; cnt[2] += ce.a[i];
     }
+}
+
+// final scoring of cell c from A, T [n_rows][K] (canonical order): what vtx_k_cl_score_pinned computes with no pinned sample
+inline void score_cell(const CellEntries& ce, uint32_t c, uint32_t K, const int64_t* A, const int64_t* T, int64_t* ll, uint64_t* cnt)
+{
+    score_cell_by(ce, c, K, [&](size_t v, uint32_t k, double* th, double* om) { theta(A[v * K + k], T[v * K + k], th, om); }, ll, cnt);
 }
 
 #ifdef __CUDACC__
@@ -412,60 +420,6 @@ __global__ void __launch_bounds__(kClThreads) vtx_k_cl_final(Perm perm, uint64_t
         int64_t sa, st;
         row_sums(col, r, a, row_start[v], row_start[v + 1], w, K, lane, k, &sa, &st);
         if (lane < K) { A[v * K + lane] = sa; T[v * K + lane] = st; }
-    }
-}
-
-// One warp per cell.  Lane k < K turns its cluster's A, T at the entry's row into theta and 1 - theta; lane l then takes the
-// two clusters of each of its hypotheses h = l + 32j (j < KH = ceil(H / 32)) by shuffle.
-template <int KH>
-__global__ void __launch_bounds__(kClThreads) vtx_k_cl_score(CellEntries ce, uint32_t n_cols, uint32_t K, const int64_t* __restrict__ A,
-                                                             const int64_t* __restrict__ T, int64_t* __restrict__ ll, uint64_t* __restrict__ cnt)
-{
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t H = donors::n_hyp(K);
-    uint32_t pair[KH];
-#pragma unroll
-    for (int j = 0; j < KH; ++j) {
-        uint32_t d1 = 0, d2 = 0;
-        if (lane + 32u * j < H) donors::hyp_donors(lane + 32u * j, K, &d1, &d2);
-        pair[j] = d1 | d2 << 8;
-    }
-    for (uint32_t c = warp; c < n_cols; c += n_warps) {
-        const uint32_t i0 = ce.start[c], i1 = ce.start[c + 1];
-        int64_t acc[KH];
-#pragma unroll
-        for (int j = 0; j < KH; ++j) acc[j] = 0;
-        uint64_t sum_r = 0, sum_a = 0;
-        for (uint32_t base = i0; base < i1; base += 32) {
-            const uint32_t i = base + lane;
-            uint32_t v = 0, r = 0, a = 0;
-            if (i < i1) { v = ce.row[i]; r = ce.r[i]; a = ce.a[i]; }
-            const uint32_t n = min(32u, i1 - base);
-            for (uint32_t e = 0; e < n; ++e) {
-                const uint32_t ve = __shfl_sync(0xffffffffu, v, e), re = __shfl_sync(0xffffffffu, r, e), ae = __shfl_sync(0xffffffffu, a, e);
-                double th = 0.5, om = 0.5;
-                if (lane < K) theta(A[size_t(ve) * K + lane], T[size_t(ve) * K + lane], &th, &om);
-#pragma unroll
-                for (int j = 0; j < KH; ++j) {
-                    const uint32_t d1 = pair[j] & 0xFF, d2 = pair[j] >> 8;
-                    const double ti = __shfl_sync(0xffffffffu, th, d1), oi = __shfl_sync(0xffffffffu, om, d1);
-                    const double tj = __shfl_sync(0xffffffffu, th, d2), oj = __shfl_sync(0xffffffffu, om, d2);
-                    if (lane + 32u * j < H) {
-                        int32_t la, lr;
-                        pair_logs(ti, oi, tj, oj, &la, &lr);
-                        acc[j] += int64_t(re) * lr + int64_t(ae) * la;
-                    }
-                }
-            }
-            sum_r += r; sum_a += a;
-        }
-        sum_r = warp_sum_u64(sum_r); sum_a = warp_sum_u64(sum_a);
-        int64_t* out = ll + size_t(c) * H;
-#pragma unroll
-        for (int j = 0; j < KH; ++j)
-            if (lane + 32u * j < H) out[lane + 32u * j] = acc[j];
-        if (lane == 0) { cnt[3 * size_t(c)] = i1 - i0; cnt[3 * size_t(c) + 1] = sum_r; cnt[3 * size_t(c) + 2] = sum_a; }
     }
 }
 #endif   // __CUDACC__

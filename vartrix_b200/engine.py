@@ -370,19 +370,40 @@ def _np_from(ptr, n, dt, copy=True):
     return a.copy() if copy else a
 
 
+def _arr(ptr, count, dtype, shape):
+    """a NumPy copy of `count` elements at a library-owned pointer (which the next call of the same kind reuses)"""
+    if count == 0:
+        return np.zeros(shape, dtype)
+    return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
+
+
+def _entries(row, col, ref, alt):
+    """the count entries (row, col, REF, ALT) as uint32 arrays, and their common length"""
+    arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
+    n = len(arrs[0])
+    if any(len(x) != n for x in arrs):
+        raise ValueError("row, col, ref and alt must have the same length")
+    return arrs, n
+
+
+def _permille(rho_permille, estimate: bool) -> int:
+    """rho_permille as the C ABI takes it: an integer m (thousandths), or with `estimate`, None as -1"""
+    if estimate and rho_permille is None:
+        return -1
+    if isinstance(rho_permille, (bool, np.bool_)) or not isinstance(rho_permille, (int, np.integer)):
+        raise TypeError(f"rho_permille must be {'None or ' if estimate else ''}an integer number of thousandths, not {rho_permille!r}")
+    return int(rho_permille)
+
+
 def _clusters_dict(out, restarts: int) -> dict:
     """NumPy copies of a vtx_clusters (library-owned memory that the next clustering call reuses)"""
-    def arr(ptr, count, dtype, shape):
-        if count == 0:
-            return np.zeros(shape, dtype)
-        return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
     nc, nh, nr, kk = int(out.n_cols), int(out.n_hyp), int(out.n_rows), int(out.k)
     return dict(k=kk, n_hyp=nh, best_restart=int(out.best_restart), rows_used=int(out.rows_used),
-                ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
-                row_used=arr(out.row_used, nr, np.uint8, (nr,)), alt_w=arr(out.alt_w, nr * kk, np.int64, (nr, kk)),
-                depth_w=arr(out.depth_w, nr * kk, np.int64, (nr, kk)),
-                restart_score=arr(out.restart_score, restarts, np.int64, (restarts,)),
-                restart_iters=arr(out.restart_iters, restarts, np.uint32, (restarts,)))
+                ll=_arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=_arr(out.counts, nc * 3, np.uint64, (nc, 3)),
+                row_used=_arr(out.row_used, nr, np.uint8, (nr,)), alt_w=_arr(out.alt_w, nr * kk, np.int64, (nr, kk)),
+                depth_w=_arr(out.depth_w, nr * kk, np.int64, (nr, kk)),
+                restart_score=_arr(out.restart_score, restarts, np.int64, (restarts,)),
+                restart_iters=_arr(out.restart_iters, restarts, np.uint32, (restarts,)))
 
 
 class Engine:
@@ -638,10 +659,7 @@ class Engine:
         -> dict of NumPy copies: ll int64[n_cols, H] (x 2^24), counts uint64[n_cols, 3], row_used uint8[n_rows],
         alt_w / depth_w int64[n_rows, k] (x 2^16), restart_score int64[restarts], restart_iters uint32[restarts], and the
         scalars k, n_hyp, best_restart, rows_used."""
-        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
-        n = len(arrs[0])
-        if any(len(x) != n for x in arrs):
-            raise ValueError("row, col, ref and alt must have the same length")
+        arrs, n = _entries(row, col, ref, alt)
         out = _capi.Clusters()
         p = _capi.ClusterParams(int(k), int(restarts), int(seed) & 0xFFFFFFFFFFFFFFFF)
         ptr = [x.ctypes.data if n else None for x in arrs]
@@ -654,17 +672,13 @@ class Engine:
         DESIGN.md §5k): count entries as cluster_cells takes them, dosage uint8[n_rows, J] (0, 1, 2 or GT_MISSING) of the J
         genotyped samples, 1 <= J <= k - 1, and the ambient fraction rho_permille / 1000 (an integer m in 0..500).  -> the dict
         cluster_cells returns; clusters 0 .. J - 1 are the samples in dosage's column order, J .. k - 1 the free clusters."""
-        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
-        n = len(arrs[0])
-        if any(len(x) != n for x in arrs):
-            raise ValueError("row, col, ref and alt must have the same length")
+        arrs, n = _entries(row, col, ref, alt)
         g = np.ascontiguousarray(dosage, dtype=np.uint8)
         if g.ndim != 2 or g.shape[0] != int(n_rows):
             raise ValueError(f"dosage must be a [n_rows, samples] array, not shape {g.shape}")
-        if isinstance(rho_permille, (bool, np.bool_)) or not isinstance(rho_permille, (int, np.integer)):
-            raise TypeError(f"rho_permille must be an integer number of thousandths, not {rho_permille!r}")
+        m = _permille(rho_permille, estimate=False)
         out = _capi.Clusters()
-        p = _capi.ClusterPinnedParams(int(k), int(restarts), int(seed) & 0xFFFFFFFFFFFFFFFF, g.shape[1], float(error_rate), int(rho_permille))
+        p = _capi.ClusterPinnedParams(int(k), int(restarts), int(seed) & 0xFFFFFFFFFFFFFFFF, g.shape[1], float(error_rate), m)
         ptr = [x.ctypes.data if n else None for x in arrs]
         self._ck(self._L.vtx_cluster_cells_pinned(self._h, n, *ptr, int(n_rows), int(n_cols), g.ctypes.data, C.byref(p), C.byref(out)),
                  "vtx_cluster_cells_pinned")
@@ -677,31 +691,22 @@ class Engine:
         fraction; an integer m in 0..500 fixes it at m / 1000 (anything else, e.g. the fraction 0.15, raises).  -> dict of NumPy copies: ll int64[n_cols, H] (x 2^24), counts
         uint64[n_cols, 3], grid_permille uint16[E], grid_objective int64[E], grid_calls uint64[E, 3] (ascending m),
         row_alt / row_depth uint64[n_rows], and the scalars rho_permille, rho (= rho_permille / 1000), n_hyp, rows_usable."""
-        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
-        n = len(arrs[0])
-        if any(len(x) != n for x in arrs):
-            raise ValueError("row, col, ref and alt must have the same length")
+        arrs, n = _entries(row, col, ref, alt)
         g = np.ascontiguousarray(dosage, dtype=np.uint8)
         if g.ndim != 2 or g.shape[0] != int(n_rows):
             raise ValueError(f"dosage must be a [n_rows, donors] array, not shape {g.shape}")
-        if rho_permille is not None and (isinstance(rho_permille, (bool, np.bool_)) or not isinstance(rho_permille, (int, np.integer))):
-            raise TypeError(f"rho_permille must be None or an integer number of thousandths, not {rho_permille!r}")
+        m = _permille(rho_permille, estimate=True)
         out = _capi.Ambient()
-        p = _capi.AmbientParams(g.shape[1], float(error_rate), -1 if rho_permille is None else int(rho_permille), int(grid_batch))
+        p = _capi.AmbientParams(g.shape[1], float(error_rate), m, int(grid_batch))
         ptr = [x.ctypes.data if n else None for x in arrs]
         self._ck(self._L.vtx_donors_ambient(self._h, n, *ptr, int(n_rows), int(n_cols), g.ctypes.data if g.size else None,
                                             C.byref(p), C.byref(out)), "vtx_donors_ambient")
-
-        def arr(ptr, count, dtype, shape):
-            if count == 0:
-                return np.zeros(shape, dtype)
-            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
         nc, nh, nr, ne = int(out.n_cols), int(out.n_hyp), int(out.n_rows), int(out.n_evaluated)
         return dict(rho_permille=int(out.rho_permille), rho=int(out.rho_permille) / 1000, n_hyp=nh, rows_usable=int(out.rows_usable),
-                    ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
-                    grid_permille=arr(out.grid_permille, ne, np.uint16, (ne,)), grid_objective=arr(out.grid_objective, ne, np.int64, (ne,)),
-                    grid_calls=arr(out.grid_calls, ne * 3, np.uint64, (ne, 3)), row_alt=arr(out.row_alt, nr, np.uint64, (nr,)),
-                    row_depth=arr(out.row_depth, nr, np.uint64, (nr,)))
+                    ll=_arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=_arr(out.counts, nc * 3, np.uint64, (nc, 3)),
+                    grid_permille=_arr(out.grid_permille, ne, np.uint16, (ne,)), grid_objective=_arr(out.grid_objective, ne, np.int64, (ne,)),
+                    grid_calls=_arr(out.grid_calls, ne * 3, np.uint64, (ne, 3)), row_alt=_arr(out.row_alt, nr, np.uint64, (nr,)),
+                    row_depth=_arr(out.row_depth, nr, np.uint64, (nr,)))
 
     def cluster_genotypes(self, clusters: dict, row_alt, row_depth, dosage=None, error_rate: float = 0.01, rho_permille=None) -> dict:
         """Genotypes of the clusters against ambient RNA and their match to genotyped samples (vtx_cluster_genotypes,
@@ -728,25 +733,19 @@ class Engine:
             if g.ndim != 2 or g.shape[0] != n_rows:
                 raise ValueError(f"dosage must be a [n_rows, samples] array, not shape {g.shape}")
         s = 0 if g is None else g.shape[1]
-        if rho_permille is not None and (isinstance(rho_permille, (bool, np.bool_)) or not isinstance(rho_permille, (int, np.integer))):
-            raise TypeError(f"rho_permille must be None or an integer number of thousandths, not {rho_permille!r}")
+        m = _permille(rho_permille, estimate=True)
         out = _capi.ClusterGt()
-        p = _capi.ClusterGtParams(k, float(error_rate), -1 if rho_permille is None else int(rho_permille), s)
+        p = _capi.ClusterGtParams(k, float(error_rate), m, s)
         ptr = [x.ctypes.data if n_rows else None for x in (A, T, used, ra, rd)]
         self._ck(self._L.vtx_cluster_genotypes(self._h, n_rows, *ptr, g.ctypes.data if g is not None and g.size else None,
                                                C.byref(p), C.byref(out)), "vtx_cluster_genotypes")
-
-        def arr(ptr, count, dtype, shape):
-            if count == 0:
-                return np.zeros(shape, dtype)
-            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
         ne, nt = int(out.n_evaluated), int(out.n_touched)
         return dict(rho_permille=int(out.rho_permille), rho=int(out.rho_permille) / 1000, rows_fit=int(out.rows_fit),
-                    rows_compared=int(out.rows_compared), grid_permille=arr(out.grid_permille, ne, np.uint16, (ne,)),
-                    grid_objective=arr(out.grid_objective, ne, np.int64, (ne,)), touched=arr(out.touched, nt, np.uint64, (nt,)),
-                    gt=arr(out.gt, nt * k, np.uint8, (nt, k)), pl=arr(out.pl, nt * k * 3, np.uint32, (nt, k, 3)),
-                    match_ll=arr(out.match_ll, k * s, np.int64, (k, s)), match_discordant=arr(out.match_discordant, k * s, np.uint64, (k, s)),
-                    match_rows=arr(out.match_rows, k, np.uint64, (k,)), match_called=arr(out.match_called, k, np.uint64, (k,)))
+                    rows_compared=int(out.rows_compared), grid_permille=_arr(out.grid_permille, ne, np.uint16, (ne,)),
+                    grid_objective=_arr(out.grid_objective, ne, np.int64, (ne,)), touched=_arr(out.touched, nt, np.uint64, (nt,)),
+                    gt=_arr(out.gt, nt * k, np.uint8, (nt, k)), pl=_arr(out.pl, nt * k * 3, np.uint32, (nt, k, 3)),
+                    match_ll=_arr(out.match_ll, k * s, np.int64, (k, s)), match_discordant=_arr(out.match_discordant, k * s, np.uint64, (k, s)),
+                    match_rows=_arr(out.match_rows, k, np.uint64, (k,)), match_called=_arr(out.match_called, k, np.uint64, (k,)))
 
     def cluster_refine(self, row, col, ref, alt, n_rows: int, n_cols: int, clusters: dict, error_rate: float = 0.01,
                        max_rounds: int = 8) -> dict:
@@ -756,10 +755,7 @@ class Engine:
         last round, label uint32[n_cols] (NO_LABEL unless singlet), rho_permille / rows_fit / n_touched / rows_scored / changed
         int64[rounds] and calls int64[rounds, 3] per round, the last round's touched uint64[n_touched], gt uint8[n_touched, k] and
         pl uint32[n_touched, k, 3], and the scalars k, n_hyp, n_rounds, converged."""
-        arrs = [np.ascontiguousarray(x, dtype=np.uint32) for x in (row, col, ref, alt)]
-        n = len(arrs[0])
-        if any(len(x) != n for x in arrs):
-            raise ValueError("row, col, ref and alt must have the same length")
+        arrs, n = _entries(row, col, ref, alt)
         A = np.ascontiguousarray(clusters["alt_w"], dtype=np.int64)
         T = np.ascontiguousarray(clusters["depth_w"], dtype=np.int64)
         used = np.ascontiguousarray(clusters["row_used"], dtype=np.uint8)
@@ -771,23 +767,18 @@ class Engine:
         ptr = [x.ctypes.data if n else None for x in arrs] + [x.ctypes.data if int(n_rows) else None for x in (A, T, used)]
         self._ck(self._L.vtx_cluster_refine(self._h, n, *ptr[:4], int(n_rows), int(n_cols), *ptr[4:], C.byref(p), C.byref(out)),
                  "vtx_cluster_refine")
-
-        def arr(ptr, count, dtype, shape):
-            if count == 0:
-                return np.zeros(shape, dtype)
-            return np.ctypeslib.as_array(ptr, shape=(count,)).astype(dtype, copy=True).reshape(shape)
         nc, nh, nt, nr = int(out.n_cols), int(out.n_hyp), int(out.n_touched), int(out.n_rounds)
         rounds = [out.rounds[i] for i in range(nr)]
         return dict(k=k, n_hyp=nh, n_rounds=nr, converged=bool(out.converged),
-                    ll=arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=arr(out.counts, nc * 3, np.uint64, (nc, 3)),
-                    label=arr(out.label, nc, np.uint32, (nc,)),
+                    ll=_arr(out.ll, nc * nh, np.int64, (nc, nh)), counts=_arr(out.counts, nc * 3, np.uint64, (nc, 3)),
+                    label=_arr(out.label, nc, np.uint32, (nc,)),
                     rho_permille=np.array([x.rho_permille for x in rounds], np.int64),
                     rows_fit=np.array([x.rows_fit for x in rounds], np.int64), n_touched=np.array([x.n_touched for x in rounds], np.int64),
                     rows_scored=np.array([x.rows_scored for x in rounds], np.int64),
                     calls=np.array([list(x.calls) for x in rounds], np.int64).reshape(nr, 3),
                     changed=np.array([x.changed for x in rounds], np.int64),
-                    touched=arr(out.touched, nt, np.uint64, (nt,)), gt=arr(out.gt, nt * k, np.uint8, (nt, k)),
-                    pl=arr(out.pl, nt * k * 3, np.uint32, (nt, k, 3)))
+                    touched=_arr(out.touched, nt, np.uint64, (nt,)), gt=_arr(out.gt, nt * k, np.uint8, (nt, k)),
+                    pl=_arr(out.pl, nt * k * 3, np.uint32, (nt, k, 3)))
 
     def last_error(self) -> str:
         return (self._L.vtx_last_error(self._h) or b"").decode()
